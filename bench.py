@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the WVA optimization hot path on B200.
+"""bench.py — headline benchmark of the WVA optimization hot path on H100.
 
-Metric (BASELINE.json): (model,variant,replica) evals/sec + solver wall-ms at 1/2/4/8 B200, next to the reference
+Metric (BASELINE.json): (model,variant,replica) evals/sec + solver wall-ms at 1/2/4/8 H100, next to the reference
 algorithm on the box's host cores.
 
 Workload = BASELINE.json configs[2], the largest single-GPU configuration: 100 k models x 32 accelerator variants x 256
@@ -23,7 +23,11 @@ A second timed leg runs BASELINE configs[3], the one HBM-bound kernel of the pat
 `roofline_hbm`).  The queueing kernels are FP64-pipe bound (SURVEY 0.4): `roofline` reports the dominant kernel (the
 sizer) against the HBM peak as the contract asks — meaningless by construction — and against the measured FP64 peak.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+--dump-outputs DIR writes, after the timed steps, what the last step computed as DIR/<name>.npy (float32 for float32
+results, float64 for everything else; fixed seeded samples of the large arrays, under 64 MB in all): a sample of the
+candidates, the limited solution, a sample of the replica grid and, after the saturation leg, a sample of its targets.
+
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 """
 from __future__ import annotations
 
@@ -58,7 +62,9 @@ CAP_FRACTION = 0.6
 ALG_BYTES_PER_EVAL = 17.9                 # SURVEY.md 8(d): 16 B written + amortised inputs per grid evaluation
 ALG_BYTES_PER_PAIR = 24 + 36.0 / A + 37   # sizing: 24 B + 36 B/A in, 37 B out per (server, accelerator)
 FP64_OPS_PER_STATE = 9.0                  # 5 FP64-pipe ops per pass-1 state, 13 per pass-2 state (DESIGN.md 4)
+HBM_PEAK_GBS = 3350.0                     # H100 SXM data sheet (HBM3); MEASURED_PEAKS.json overrides it
 METRIC = "(model,variant,replica) evals/sec"
+DUMP_SAMPLE = 1 << 18                     # indices drawn per sampled output array (--dump-outputs)
 
 
 def workload(scale: float = 1.0):
@@ -104,7 +110,7 @@ def effective_cores():
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (profiling recipe)."""
+    """nvidia-smi clocks / throttle reasons / power limit during the timed region (profiling recipe)."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -113,7 +119,7 @@ class ClockSampler(threading.Thread):
     def run(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.index}", f"--query-gpu={q}",
                                           "--format=csv,noheader,nounits", "-lms", "50"],
@@ -126,7 +132,7 @@ class ClockSampler(threading.Thread):
     def stop(self):
         if self.proc:
             self.proc.terminate()
-        sm, smax, reasons = [], 0.0, set()
+        sm, smax, reasons, plim = [], 0.0, set(), None
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
@@ -134,10 +140,62 @@ class ClockSampler(threading.Thread):
                 for n, v in zip(names, r[3:7]):
                     if v.lower().startswith("active"):
                         reasons.add(n)
+                plim = float(r[7])
             except Exception:
                 continue
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": smax or None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": plim, "reasons": sorted(reasons), "samples": len(sm)}
+
+
+# ---- --dump-outputs ---------------------------------------------------------------------------------------------------
+def _sample(n: int, stream: int, k: int = DUMP_SAMPLE):
+    """a fixed, seeded sample of k of n flat indices (sorted, no repeats); every index when n <= k"""
+    if n <= k:
+        return np.arange(n)
+    return np.unique(np.random.default_rng(stream).integers(0, n, k))
+
+
+def _save(out_dir: str, arrays: dict):
+    """float32 results as float32, everything else as float64 (exact for the integer and flag results)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        dt = np.float32 if a.dtype == np.float32 else np.float64
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=dt))
+
+
+def dump_queueing(eng, out_dir: str):
+    """What the last resident step left on the device: the candidates of calculate(), the solution of the limited solve
+    and the materialised replica grid (this rank's block), sampled at fixed seeded indices."""
+    cand, sol = eng.candidates(), eng.solution()
+    pairs = _sample(cand["state"].size, 1)
+    out = {"candidates_index": pairs}
+    out.update({"candidates_" + k: v.reshape(-1)[pairs] for k, v in cand.items()})
+    out.update({"solution_" + k: v for k, v in sol.items()})
+    front = eng.grid_fetch_frontier().reshape(-1)
+    fpairs = _sample(front.size, 1)
+    out["grid_frontier_index"], out["grid_frontier"] = fpairs, front[fpairs]
+    n = (eng.hi - eng.lo) * eng.A * R
+    cells = _sample(n, 2, 2 * DUMP_SAMPLE)
+    out["grid_index"] = cells
+    buf = np.empty(max(n, 1) * 4, np.uint8)          # one field of the whole grid at a time
+    for i, (k, dt) in enumerate((("ok", np.uint8), ("ttft", np.float32), ("itl", np.float32), ("rho", np.float32),
+                                 ("tput", np.float32))):
+        a = buf[: n * np.dtype(dt).itemsize].view(dt)
+        ptrs = [None] * 6
+        ptrs[i] = a.ctypes.data
+        eng._check(eng.lib.wva_grid_fetch(eng.ctx, *ptrs), "wva_grid_fetch")
+        out["grid_" + k] = a[cells]
+    _save(out_dir, out)
+
+
+def dump_saturation(eng, out_dir: str):
+    """What the last saturation run returns to a caller (saturation_fetch without detail), sampled."""
+    res = eng.saturation_fetch(fields=("var_target", "mod_flags", "partials", "partials_all"))
+    var, mod = _sample(res["var_target"].size, 3), _sample(res["mod_flags"].size, 4)
+    _save(out_dir, {"saturation_var_index": var, "saturation_var_target": res["var_target"][var],
+                    "saturation_mod_index": mod, "saturation_mod_flags": res["mod_flags"][mod],
+                    "saturation_partials": res["partials"], "saturation_partials_all": res["partials_all"]})
 
 
 # ---- the reference algorithm on the host cores ------------------------------------------------------------------------
@@ -237,6 +295,7 @@ def main():
     ap.add_argument("--scale", type=float, default=1.0, help="shrink the system (development only; 1.0 = configs[2])")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-saturation", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -344,13 +403,15 @@ def main():
         dist.all_reduce(cnt)
     ph = dict(zip(keys, ph.tolist()))
     size_solves, size_states, grid_solves, grid_states = cnt.tolist()
+    if args.dump_outputs and rank == 0:
+        dump_queueing(eng, args.dump_outputs)
 
     # ---- end-to-end arm ---------------------------------------------------------------------------------------------------
     for _ in range(2):
         e2e_step()
     barrier()
     e0.record()
-    e2e_steps = max(2, args.steps // 2)
+    e2e_steps = args.steps
     for _ in range(e2e_steps):
         sol, fr = e2e_step()
     e1.record()
@@ -384,13 +445,15 @@ def main():
             eng.saturation_run(False)
         ks, xs = [], []
         barrier()
-        for _ in range(max(args.steps, 5)):
+        for _ in range(args.steps):
             flush.zero_()
             torch.cuda.synchronize()      # the flush runs on torch's stream, the kernel on the library's: no overlap
             eng.saturation_run(False)
             t = eng.timing()
             ks.append(t["saturation_ms"]); xs.append(t["exchange_ms"])
         res = eng.saturation_fetch(fields=("partials", "partials_all"))
+        if args.dump_outputs and rank == 0:
+            dump_saturation(eng, args.dump_outputs)
         alg_loc = batch["n_replicas"] * 16 + batch["n_variants"] * 32 + M_loc * 40      # SURVEY 8(d)
         v = torch.tensor([float(np.mean(ks)), float(np.min(ks)), float(np.mean(xs))], dtype=torch.float64, device=dev)
         tot = torch.tensor([float(alg_loc), float(batch["n_replicas"])], dtype=torch.float64, device=dev)
@@ -403,17 +466,13 @@ def main():
                "partials_all": [int(x) for x in res["partials_all"]]}
 
     if rank == 0:
-        peaks, traffic = {}, {}
+        peaks = {}
         try:
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        except Exception:
-            pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+        hbm_peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
+        peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet"
         calc_ms, grid_ms = ph["calc_ms"], ph["grid_ms"]
         dominant = {1: "sizer_warp_kernel", 2: "sizer_lane_kernel", 3: "sizer_lane_kernel", 4: "sizer_pool_kernel"}.get(sizer_id, "sizer_lane_kernel")
         alg_bytes = S_loc * A * ALG_BYTES_PER_PAIR
@@ -439,13 +498,12 @@ def main():
                                        "chain solve (as QueueAnalyzer.Analyze does): grid_admitted_solves ran a chain"},
             "greedy": {"events": int(infos[-1]["greedy_events"]), "heap_pushes": int(infos[-1]["greedy_heap_pushes"])},
             "roofline": {"bound": "hbm", "kernel": dominant, "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
-                         "frac": achieved / hbm_peak, "traffic": traffic.get(dominant), "peak_source": peak_src,
+                         "frac": achieved / hbm_peak, "peak_source": peak_src,
                          "note": "dominant kernel of the step; algorithmic bytes / kernel time as the contract asks, but "
                                  "this kernel is FP64-pipe bound (1e3-1e5 flop/B): see `fp64`; the HBM-bound kernel of "
                                  "the path is reported in `roofline_hbm`",
                          "fp64": {"achieved_ops_per_s": fp64_rate, "peak_dfma_per_s": dfma, "peak_ddiv_per_s": ddiv,
                                   "frac_of_dfma_peak": fp64_rate / dfma,
-                                  "pipe_active_pct_ncu": (traffic.get("fp64_pipe_active_pct") or {}).get(dominant),
                                   "note": "ALGORITHMIC FP64-pipe ops (9 x live states) / kernel time on rank 0's share; "
                                           "peaks measured in this run by wva_microbench_fp64"}},
             "e2e": {"value": e2e_value, "unit": "evals/s", "h2d_bytes_per_step": int(h2d),
@@ -453,6 +511,7 @@ def main():
                     "note": "Engine.optimize (load_system from pinned host buffers -> calculate -> limited solve -> "
                             "solution to the host) + frontier-only grid + frontier to the host"},
             "gpu_launches": int(launches),
+            "gpu": torch.cuda.get_device_name(dev),
             "clocks": clocks,
             "decisions": {"allocated_limited": int((sol["state"] == 1).sum()),
                           "gpus_by_type_limited": np.asarray(sol["type_count"]).tolist(), "cap_by_type": cap.tolist()},
@@ -463,7 +522,7 @@ def main():
             line["saturation"] = sat
             line["roofline_hbm"] = {"bound": "hbm", "kernel": "saturation_kernel", "achieved": a,
                                     "peak": hbm_peak * world, "unit": "GB/s", "frac": a / (hbm_peak * world),
-                                    "traffic": traffic.get("saturation_kernel"), "peak_source": peak_src,
+                                    "peak_source": peak_src,
                                     "note": "configs[3]: algorithmic bytes of all ranks (16 B/replica + 32 B/variant + "
                                             "40 B/model) / mean kernel time (max over ranks, CUDA events on the library's "
                                             "stream, L2 flushed before every launch); peak = per-GPU copy bandwidth x ranks"}

@@ -1,5 +1,5 @@
 /*
- * wva_b200.h — C-ABI of the B200-native WVA optimization hot path.
+ * wva_b200.h — C-ABI of the H100-native (sm_90a) WVA optimization hot path.
  *
  * This is the drop-in boundary a cgo shim binds (see INTEGRATION.md and
  * llm-d-workload-variant-autoscaler_b200/go/).  The reference
@@ -37,7 +37,7 @@ enum {
   WVA_OK = 0,
   WVA_ERR_ARG = 1,        /* null pointer / negative size / inconsistent index */
   WVA_ERR_CUDA = 2,       /* a CUDA runtime call or kernel failed              */
-  WVA_ERR_NO_DEVICE = 3,  /* no usable sm_100 device (no CPU fallback exists)  */
+  WVA_ERR_NO_DEVICE = 3,  /* no usable sm_90 device (no CPU fallback exists)   */
   WVA_ERR_STATE = 4,      /* call order violated (e.g. solve before calculate) */
   WVA_ERR_NOMEM = 5,      /* host or device allocation failed                  */
   WVA_ERR_LIMIT = 6       /* a size exceeds what the kernels support           */
@@ -529,7 +529,7 @@ int32_t wva_pipeline_v2(wva_ctx* ctx, const wva_saturation_v2_in* in, const doub
 /* ---- host memory ----------------------------------------------------------- */
 /* Page-locked host buffers for the caller's SoA arrays (the collector writes its batch straight into them): every
  * entry point copies from / to such a buffer by DMA at link speed instead of through the driver's pageable staging
- * (31 MB of replica metrics: 2.4 ms pageable, 0.6 ms pinned).  Any host pointer is accepted everywhere — this is an
+ * (several times faster for a batch of replica metrics).  Any host pointer is accepted everywhere — this is an
  * optimisation, not a requirement.  Not tied to a context; free with wva_host_free. */
 int32_t wva_host_alloc(size_t bytes, void** out);
 int32_t wva_host_free(void* p);

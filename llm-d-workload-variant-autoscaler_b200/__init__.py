@@ -1,6 +1,6 @@
-"""B200-native WVA optimization hot path (queueing sizer, allocator, saturation model, limiter).
+"""H100-native WVA optimization hot path (queueing sizer, allocator, saturation model, limiter).
 
-The compute lives in csrc/ (hand-written sm_100a CUDA behind the C-ABI of
+The compute lives in csrc/ (hand-written sm_90a CUDA behind the C-ABI of
 include/wva_b200.h).  This package is the Python binding used by tests/ and
 bench.py; the Go binding a maintainer would add is shown in INTEGRATION.md.
 There is no CPU fallback: constructing an Engine without the built CUDA library

@@ -1,4 +1,4 @@
-"""ctypes image of include/wva_b200.h (the C-ABI of the B200 hot path).
+"""ctypes image of include/wva_b200.h (the C-ABI of the H100 hot path).
 
 Only struct layouts, constants and numpy<->pointer helpers live here; nothing in
 this module computes anything.  Both the product wrapper (``engine.py``) and the

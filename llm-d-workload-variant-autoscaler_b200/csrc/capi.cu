@@ -194,7 +194,7 @@ int32_t wva_create(int32_t device, wva_ctx** out) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0 || device < 0 || device >= n) return WVA_ERR_NO_DEVICE;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return WVA_ERR_NO_DEVICE;
-  if (prop.major < 10) return WVA_ERR_NO_DEVICE;  // kernels are built for sm_100a only
+  if (prop.major != 9 || prop.minor != 0) return WVA_ERR_NO_DEVICE;  // kernels are built for sm_90a only
   if (cudaSetDevice(device) != cudaSuccess) return WVA_ERR_NO_DEVICE;
   wva_ctx* ctx = new (std::nothrow) wva_ctx();
   if (!ctx) return WVA_ERR_NOMEM;
@@ -368,11 +368,9 @@ static cudaError_t launch_sizer(wva_ctx* ctx, int blocks, size_t smem, unsigned 
     // length-sorted queue: float32 probe -> (N, expected chain length) keys -> descending radix sort of the item ids
     const unsigned* order = nullptr;
     const unsigned long long n_items = split ? 2 * n_pairs : n_pairs;
-    // measured (r1, B200): the sorted queue + gang refill pays between ~130 and ~1500 pairs per SM (the items then fill
-    // 1.5-15 waves and longest-first ordering shortens the tail: -18 % at 24 k pairs, -30 % at 48 k, -15 % at 100-130 k);
-    // below, every lane holds one item and the probe is pure overhead; far above, the gain (6 % at 320 k pairs, 2 % at
-    // N = 256) no longer covers the probe's variance
-    // r2, table in global memory, 3.2 M pairs at N = 256: 402 ms natural order, 371 ms sorted + gang refill
+    // the sorted queue + gang refill pays between ~130 and ~1500 pairs per SM (the items then fill 1.5-15 waves and
+    // longest-first ordering shortens the tail); below, every lane holds one item and the probe is pure overhead; far
+    // above, the gain no longer covers the probe's variance.  With the table in global memory it is kept at any size.
     const bool by_size = n_pairs > (unsigned long long)ctx->sm_count * 130 &&
                          (n_pairs <= (unsigned long long)ctx->sm_count * 1500 || !SMEM);
     const bool do_sort = ctx->length_sort < 0 ? by_size : ctx->length_sort != 0;
@@ -484,15 +482,14 @@ int32_t wva_calculate(wva_ctx* ctx) {
     // as needed instead of filling the first SMs (lanes pull one pair each from the queue)
     // mid-size systems (measured: up to ~200 pairs per SM) still leave lanes idle: split every pair into a
     // TTFT item and an ITL item, which halves the chain of dependent solves per work item
-    // measured crossovers on B200 (natural queue order, r1): split items up to ~180 pairs per SM, split items with a
-    // speculative second chain (mode 5) up to ~380, whole pairs (mode 2, the searches share evaluations) beyond
+    // crossovers (natural queue order): split items up to ~180 pairs per SM, split items with a speculative second
+    // chain (mode 5) up to ~380, whole pairs (mode 2, the searches share evaluations) beyond
     if (!ctx->force_lane_sizer)
       ctx->lane_sizer_mode = (n_pairs <= (unsigned long long)ctx->sm_count * 180) ? 4
                            : (n_pairs <= (unsigned long long)ctx->sm_count * 380) ? 5 : 2;
     // large systems: the pool sizer (sizer_pool_kernel.cuh) regroups the pending solves of 1024 pairs per SM by
-    // length every time a warp goes back for work (88-92 % live lane-steps instead of 49-62 %)
-    // measured (B200, N = 256, pairs -> pool / lane ms): 96 k 16.0 / 16.5, 200 k 25.4 / 28.2, 400 k 40.7 / 52.6, 800 k 73.9 / 98.6,
-    // 1.6 M 140 / 190, 3.2 M 271 / 372
+    // length every time a warp goes back for work (88-92 % live lane-steps instead of 49-62 %); it overtakes the lane
+    // sizer from ~640 pairs per SM
     const bool pool_auto = !ctx->force_lane_sizer && n_pairs > (unsigned long long)ctx->sm_count * 640 && nmax <= 4096;
     if (pool_auto || (ctx->force_lane_sizer && ctx->lane_sizer_mode == 6)) {
       const int P = POOL_PMAX;
@@ -535,9 +532,9 @@ int32_t wva_calculate(wva_ctx* ctx) {
         ctx->timing.sizer_kernel = 1;
       }
     } else
-    // Head table placement (measured, B200, 320 k pairs): N = 256 leaves 192 lanes per SM in shared memory (1.5 warps per
-    // scheduler) -> 60.6 ms, against 45.4 ms with the table in global memory / L2 and two 256-thread blocks per SM under
-    // a 128-register cap; at N = 128 (384 lanes in shared memory) and N = 64 shared memory wins (19.5 vs 21.0, 9.8 vs 10.5).
+    // Head table placement: N = 256 leaves 192 lanes per SM in shared memory (1.5 warps per scheduler), slower than the
+    // table in global memory / L2 with two 256-thread blocks per SM under a 128-register cap; at N = 128 (384 lanes in
+    // shared memory) and N = 64 shared memory wins.
     if (best_per_sm >= 1 && ctx->table_mode != 2 && (ctx->table_mode == 1 || best_threads * best_per_sm > 256 || n_pairs <= (unsigned long long)ctx->sm_count * 512)) {
       int blocks = ctx->sm_count * best_per_sm;
       size_t smem = per_lane * best_threads;
@@ -594,8 +591,8 @@ static int32_t solve_view(wva_ctx* ctx, const SysView& sv, const CandView& cv, c
     } else {
       long long gstats[2] = {0, 0};
       // the static-order sweep (greedy_sweep.cuh) wherever it applies; the literal queue otherwise or on request.
-      // Measured (100 k servers x 32, capacity 60 %): 20 ms (sweep, every policy) vs 67 ms (queue, policy None) and
-      // 275 ms (queue, best-effort policies)
+      // (100 k servers x 32, capacity 60 %: the sweep is several times faster than the queue, more so under the
+      // best-effort policies)
       const bool sweep = greedy_sweep_covers(sv) && ctx->greedy_mode != 1;
       int32_t rc = sweep ? run_solve_greedy_sweep(sv, cv, ov, ctx->delayed, ctx->policy, &ctx->greedy_ws.p,
                                                   &ctx->greedy_ws.cap, ctx->stream, &ctx->launches, gstats)

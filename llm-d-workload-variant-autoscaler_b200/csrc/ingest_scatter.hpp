@@ -5,18 +5,16 @@
 // of a pod overwrites an earlier one; a sample with slot < 0 (no pod label / unknown pod) is skipped; slot >= S is an
 // argument error.
 //
-// A response in registry order is written by the plain serial loop (1.3 ms for 1.4 M samples).  A response in arbitrary pod
-// order costs that loop a cache miss per sample (14 ms per vector), so it goes through a two-pass radix partition over T
-// host threads:
+// A response in registry order is written by the plain serial loop.  A response in arbitrary pod order costs that loop a
+// cache miss per sample, so it goes through a two-pass radix partition over T host threads:
 //   pass 1  thread t takes the t-th contiguous chunk of the samples and bins them by slot range (B ranges of 2^shift
 //           <= 64 K slots) into its own segment of a scratch array — sequential reads, B sequential write streams;
 //   pass 2  range b is owned by ONE thread, which replays the bins (0, b), (1, b), … (T-1, b) in that order — i.e. in
 //           sample order, so duplicates resolve exactly as in the serial loop — and scatters into a range that fits its
 //           L2.  No two threads write the same slot (or the same 64-byte line of `has`: shift >= 6).
-// Measured on the GPU box (16-CPU quota, two sockets), 1.44 M samples in random order: 14 ms serial, 2.7 ms with 8 threads.
 // The price: the columns are the page-locked arena the cycle's H2D copy reads, and lines left dirty in the caches of
-// cores all over the host slow that DMA down (the captured graph: 0.81 -> 2.4 ms per batch); doing pass 2 on the calling
-// thread alone keeps the graph at 0.81 ms but takes 11 ms per vector, so the threads win (tools/cfg5_ingest.py).
+// cores all over the host slow that DMA down; doing pass 2 on the calling thread alone avoids that but is much slower
+// per vector, so the threads win (tools/cfg5_ingest.py compares the two).
 #pragma once
 #include <atomic>
 #include <cstdint>

@@ -70,7 +70,7 @@ __device__ __forceinline__ bool v2_replica(const SatV2In& in, int r, double kv_t
 // (c = 0, 1, 2; the other lanes wait) runs chain c as 32 dependent adds fed by LDS — 2 instructions per
 // element for the warp instead of the 14 of a shuffle-fed walk.  A slot that must not count holds +0.0 (x + 0.0 == x).
 // V2_COL = 34 doubles puts the three columns 4 banks apart: with 32 (same banks) every read was a 3-way conflict, and
-// those reads were most of the kernel's L1TEX time (ncu: 1.6e8 conflict cycles per launch at 200 000 models).
+// those reads were most of the kernel's L1TEX time.
 #define V2_COL 34
 __device__ __forceinline__ void ordered_sums3(double* buf, int lane, double a, double b, double c, double& sa, double& sb, double& sc) {
   const unsigned full = 0xffffffffu;
@@ -80,8 +80,8 @@ __device__ __forceinline__ void ordered_sums3(double* buf, int lane, double a, d
   const double2* col = reinterpret_cast<const double2*>(buf + V2_COL * (lane % 3));   // 16-byte aligned: V2_COL is even
   double acc = (lane % 3 == 0) ? sa : ((lane % 3 == 1) ? sb : sc);
   // only lanes 0-2 run the chains: with all 32 lanes shadowing them these 128-bit shared loads (one wavefront per
-  // quarter-warp) were half of the L1 data-pipe wavefronts of the kernel (ncu, r1); the kernel time did not move
-  // (0.66 ms either way) — it is bound by issue slots and latency, not by the L1 pipe
+  // quarter-warp) were half of the L1 data-pipe wavefronts of the kernel; the kernel time did not move — it is bound
+  // by issue slots and latency, not by the L1 pipe
   if (lane < 3) {
 #pragma unroll
     for (int l = 0; l < 16; l++) { const double2 t = col[l]; acc = d_add(d_add(acc, t.x), t.y); }
@@ -93,19 +93,19 @@ __device__ __forceinline__ void ordered_sums3(double* buf, int lane, double a, d
 // Replicas of one model staged per warp: a model's replicas are one contiguous range of the replica arrays, so the
 // warp reads them COALESCED (lane = replica, 5 input streams, 4 output streams), leaves (effective, demand) in shared
 // memory, and the per-variant parts — ordered demand sum, median — run lane-per-variant on shared memory.  Reading the
-// replica arrays lane-per-variant straight from global memory (12 sectors per request) kept L1TEX 93 % busy and the
-// kernel at 2.0 TB/s; staged, with conflict-free ordered sums and two rounds of loads in flight, it runs at 4.0 TB/s
-// (profiles/r1_v2_pipeline.json).  Models with more than V2_STAGE replicas still take the lane-per-variant path.
+// replica arrays lane-per-variant straight from global memory (12 sectors per request) kept L1TEX busy at half the
+// bandwidth of the staged form, with conflict-free ordered sums and two rounds of loads in flight.  Models with more
+// than V2_STAGE replicas still take the lane-per-variant path.
 #define V2_STAGE 256
 #define V2_NO_DATA 0x7fffffffffffffffLL   // never a real effective capacity: go_int64 < 2^63 - 1, and eff <= k1
 
-// 4 blocks per SM = 64 registers: measured 0.68 ms at 200 000 models x 32 variants against 0.98 / 0.77 / 0.80 ms for
-// 1 / 3 / 5 blocks (88 / 72 / 48 registers) — occupancy against spills.
+// 4 blocks per SM = 64 registers: faster than 1 / 3 / 5 blocks (88 / 72 / 48 registers) at 200 000 models x 32
+// variants — occupancy against spills.
 #ifndef V2_MINB
 #define V2_MINB 4
 #endif
 #ifndef V2_ROUNDS
-#define V2_ROUNDS 2   // rounds of replica loads in flight per lane in the staging phase (1: 0.85 ms, 2: 0.68, 3: 0.67)
+#define V2_ROUNDS 2   // rounds of replica loads in flight per lane in the staging phase (3 gains nothing over 2)
 #endif
 __global__ void __launch_bounds__(256, V2_MINB) saturation_v2_kernel(SatV2In in, SatV2Out out) {
   const unsigned full = 0xffffffffu;

@@ -189,7 +189,7 @@ sizer_lane_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
 // The plain lane kernel with its table in global memory — large N on large systems (BASELINE config 3) — is launched
 // two blocks per SM; left alone ptxas gives it 168 registers and the second block never becomes resident.  Capped at
 // 128 registers (spills only around the solver call, none in the chunk loops) both blocks run: 4 warps per SMSP feed
-// the FP64 pipe instead of 2 — measured 60.7 -> 50.6 ms on 10 000 servers x 32 accelerators, N = 256.
+// the FP64 pipe instead of 2.
 __global__ void __launch_bounds__(256, 2)
 sizer_lane_kernel_gtab_2blk(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
                             SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {

@@ -1,8 +1,8 @@
-// wva_core.cuh — device core of the B200 WVA hot path: service-time closed forms,
+// wva_core.cuh — device core of the H100 WVA hot path: service-time closed forms,
 // the state-dependent birth-death chain solver, the float32 bisection sizer and
 // CreateAllocation, written as per-lane state machines.
 //
-// The same source compiles for the device (nvcc, sm_100a) and — for logic tests
+// The same source compiles for the device (nvcc, sm_90a) and — for logic tests
 // only (tests/host_emul) — for the host, where every wrapper below maps to the
 // IEEE operation it stands for.  The product never runs the host build.
 //

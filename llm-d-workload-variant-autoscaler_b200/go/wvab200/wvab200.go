@@ -1,6 +1,6 @@
-// Package wvab200 is the cgo shim that binds the B200 hot path (include/wva_b200.h) behind the
-// reference's own Go seams.  COMPILE-UNVERIFIED: neither the build container nor the GPU box has a Go
-// toolchain (`go: command not found`), so this file has never been compiled; it documents, in code, the
+// Package wvab200 is the cgo shim that binds the H100 hot path (include/wva_b200.h) behind the
+// reference's own Go seams.  COMPILE-UNVERIFIED: the project's build has no Go toolchain, so this file
+// has never been compiled; it documents, in code, the
 // binding a maintainer adds.  Build needs CGO_ENABLED=1 (the reference's Dockerfile:25 uses 0), glibc,
 // libcudart and libwva_b200.so on the loader path.
 //
@@ -46,8 +46,7 @@ func New(device int) (*Ctx, error) {
 func (x *Ctx) Close() { C.wva_destroy(x.c) }
 
 // PinnedFloat64 / PinnedInt64 return slices over page-locked C memory (wva_host_alloc): a collector that writes its
-// per-replica SoA batch into them gets DMA at link speed through every entry point (BASELINE config 5: 6.9 -> 2.1 ms per
-// 10 k-model batch).  The memory is C memory — cgo's pointer rules do not apply — and lives until Free.
+// per-replica SoA batch into them gets DMA at link speed through every entry point (BASELINE config 5).  The memory is C memory — cgo's pointer rules do not apply — and lives until Free.
 type Pinned struct{ p unsafe.Pointer }
 
 func PinnedBytes(n int) (*Pinned, error) {

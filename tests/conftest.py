@@ -13,7 +13,7 @@ PKG_NAME = "llm-d-workload-variant-autoscaler_b200"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -1,5 +1,5 @@
-import importlib, sys, time, numpy as np
-sys.path.insert(0,'/root/repo')
+import importlib, os, sys, time, numpy as np
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 pkg = importlib.import_module("llm-d-workload-variant-autoscaler_b200")
 with pkg.Engine(0) as e:
     rows=[]

@@ -1,6 +1,6 @@
 // Microbenchmark: FP64 DFMA throughput per SM as a function of warps per SM and independent chains per thread.
-// Answers: what is the dependent-issue latency of DFMA on B200, and how many chains x warps saturate the pipe?
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_ilp fp64_ilp.cu ; run: ./fp64_ilp
+// Answers: what is the dependent-issue latency of DFMA on H100, and how many chains x warps saturate the pipe?
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_ilp fp64_ilp.cu ; run: ./fp64_ilp
 #include <cstdio>
 #include <cuda_runtime.h>
 

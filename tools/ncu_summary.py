@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (raw page) into the handful of numbers DESIGN.md / profiles/ quote."""
+"""Summarise an .ncu-rep (raw page) into the handful of numbers a kernel review quotes."""
 import csv, subprocess, sys
 rep = sys.argv[1]
 out = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout
