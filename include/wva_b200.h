@@ -168,6 +168,8 @@ typedef struct wva_timing {
                               shared memory), 3 lane per pair (table in global memory), 4 pool sizer; 0 nothing to size */
   int64_t greedy_heap_pushes; /* entries the last limited wva_solve pushed into the re-insertion heap (greedy.go:143-163) */
   int64_t greedy_events;      /* head entries the last limited wva_solve processed (greedy.go:112-165 loop trips)    */
+  int64_t certify_fallbacks;  /* chain solves of the last calculate/grid whose certified fast solve (DESIGN.md §3 E12)
+                                 could not prove the reference's float32 results and that the exact solver redid      */
 } wva_timing;
 
 /* ---- lifecycle ----------------------------------------------------------- */

@@ -74,7 +74,7 @@ class Timing(C.Structure):
                 ("grid_ms", C.c_float), ("saturation_ms", C.c_float), ("limit_ms", C.c_float),
                 ("d2h_ms", C.c_float), ("chain_solves", C.c_int64), ("chain_states", C.c_int64),
                 ("overflow_pairs", C.c_int64), ("exchange_ms", C.c_float), ("sizer_kernel", C.c_int32),
-                ("greedy_heap_pushes", C.c_int64), ("greedy_events", C.c_int64)]
+                ("greedy_heap_pushes", C.c_int64), ("greedy_events", C.c_int64), ("certify_fallbacks", C.c_int64)]
 
 
 class SaturationIn(C.Structure):

@@ -564,7 +564,11 @@ sizer_done:
   if (getenv("WVA_SIZER_DEBUG") && hc.lockstep_slots)
     fprintf(stderr, "sizer: live lane-steps %llu of %llu lock-step slots (%.1f %%)\n", hc.states, hc.lockstep_slots,
             100.0 * (double)hc.states / (double)hc.lockstep_slots);
+  if (getenv("WVA_SIZER_DEBUG"))
+    fprintf(stderr, "sizer: %llu of %llu chain solves not certified (E12), redone by the exact solver\n", hc.certify_fallbacks,
+            hc.solves);
   ctx->timing.overflow_pairs = (int64_t)hc.overflow_pairs;
+  ctx->timing.certify_fallbacks = (int64_t)hc.certify_fallbacks;
   if (hc.limit_hit) { ctx->last_error = "a (server, accelerator) pair needs a max batch size above 65536"; return WVA_ERR_LIMIT; }
   if (hc.overflow_pairs) {
     // float64 overflow-rescale branch (mm1modelstatedependent.go:84-89,96-104): exact slow path

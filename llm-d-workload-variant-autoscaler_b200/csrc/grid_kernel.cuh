@@ -26,6 +26,7 @@ struct GridCounters {
   int limit_hit, pad_;
   unsigned long long slots0, slots_rest, rounds;   // 32 x longest chain of the round: first round of a pair / later rounds
   unsigned long long slots_def;                   // the same for the deferred pass
+  unsigned long long certify_fallbacks;           // deferred pass: fast solves (E12) redone by the exact solver
 };
 
 // Deferral of the near-saturation levels (large systems).  A pair's chain length is a steep function of lambda / mu_N
@@ -287,7 +288,9 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
     bool bad = false, ovf = false;
     if (uniform) {
       TileTable tt; tt.rows = df.rows; tt.row_stride = df.row_stride; tt.slot = (int)pair; tt.tile = tile; tt.n_head = nref - 1;
-      lockstep_solve(m, tt, lambda, live, st, sv, bad);
+      sv = lockstep_solve_fast(m, tt, lambda, live, st, &ctr->certify_fallbacks);
+      bad = sv < 0;
+      if (bad) sv = -1 - sv;
     } else if (live) {
       Chain c;
       chain_start(c, lambda);

@@ -46,9 +46,6 @@ struct LaneTable {   // one float32 column per lane ([n][thread], bank = lane); 
 // cp.async (row by row: each row a coalesced 128-byte access, no registers, no scoreboard) while the lanes work on
 // tile k, so the only exposed latency is the first tile of a pass.
 struct TileTable {
-#ifndef WVA_TILE_CHUNK
-#define WVA_TILE_CHUNK 16
-#endif
   static constexpr int kChunk = WVA_TILE_CHUNK;   // states per unrolled chunk of the solver (code size vs loop overhead)
   const float* rows;      // base of the CTA's rows
   int row_stride;         // floats per row (a multiple of 32, >= N)
@@ -454,6 +451,99 @@ template <class Tab>
 __device__ __forceinline__ void lockstep_solve(const PairModel& m, const Tab& tab, float lambda, bool active,
                                                SolveStats& st, int& states, bool& bad) {
   lockstep_solve_n<1, Tab>(m, tab, &lambda, &active, &st, states, bad);
+}
+
+// ---- (E12) certified fast solve: one head pass per lane, closed-form tail, exact solver for the rest --------------
+// Head chunk, software-pipelined like p1_chunk (stage s of state j at slot 3j + s):
+//   0: x = p*lam, q0 = p*lamr (+ exponent window)   1: rem   2: p'   3: sum += p', T = fma(j, p', T)
+//   4: m = min(2^-53 sum, p')   5: A += m
+template <int CH>
+__device__ __forceinline__ void fast_chunk(FastHead& h, double lam, const double (&mu)[CH], const double (&r)[CH], double dn,
+                                           int& mn, int& mx) {
+  double x[CH], q0[CH], rem[CH], pn[CH + 1], sm[CH + 1], mm[CH], lamr[CH];
+  pn[0] = h.p; sm[0] = h.sum;
+#pragma unroll
+  for (int j = 0; j < CH; j++) lamr[j] = d_mul(lam, r[j]);
+#pragma unroll
+  for (int slot = 0; slot < 3 * CH + 3; slot++) {
+#pragma unroll
+    for (int j = 0; j < CH; j++) {
+      const int st = slot - 3 * j;
+      if (st == 0) {
+        x[j] = d_mul(pn[j], lam);
+        q0[j] = d_mul(pn[j], lamr[j]);
+        const int hw = d_hi(x[j]);
+        mn = min(mn, hw); mx = max(mx, hw);
+      }
+      if (st == 1) rem[j] = d_fma(-q0[j], mu[j], x[j]);
+      if (st == 2) pn[j + 1] = d_fma(rem[j], r[j], q0[j]);
+      if (st == 3) { sm[j + 1] = d_add(sm[j], pn[j + 1]); h.T = d_fma(d_add(dn, (double)(j + 1)), pn[j + 1], h.T); }
+      if (st == 4) mm[j] = d_min(d_mul(sm[j + 1], 0x1p-53), pn[j + 1]);
+      if (st == 5) h.A = d_add(h.A, mm[j]);
+    }
+  }
+  h.p = pn[CH]; h.sum = sm[CH];
+}
+
+// One solve per lane at `lambda` (inactive lanes ride along): the fast head pass for every active lane, the closed-form
+// tail and certification (fast_solve_finish), then the exact lockstep_solve for the lanes that were not certified.
+// Returns the states visited (the fallback's included), or -1 - states when the solve is `bad` as for lockstep_solve (by
+// value: out-parameters cost the callers stack and spills).  Every lane that takes the exact solver adds 1 to *fallbacks
+// (rare: a counter in registers would be live across the caller's whole loop).
+template <class Tab>
+__device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& tab, float lambda, bool active, SolveStats& st,
+                                                unsigned long long* fallbacks) {
+  constexpr int CH = Tab::kChunk;
+  static_assert(CH == WVA_TILE_CHUNK, "the head pass exits at the chunk boundaries the host replay (fast_solve) uses");
+  const unsigned full = 0xffffffffu;
+  const int NH = m.N - 1;
+  double lam = active ? (double)lambda : 0.0;
+  FastHead h;
+  h.p = 1.0; h.sum = 1.0; h.T = 0.0; h.A = 0.0; h.n = 0; h.ok = true; h.exited = false;
+  bool live = active;
+  int states = 0, n = 0;
+  double p_exit = 0.0;
+  while (n < NH && __any_sync(full, live)) {
+    const int cnt = min(CH, NH - n);
+    tab.prepare(n);
+    const double mu0 = tab.mu_at(n);
+    int mn = 0x7fffffff, mx = 0;
+    if (cnt == CH) {
+      double mu[CH], r[CH];
+#pragma unroll
+      for (int j = 0; j < CH; j++) tab.load(n + j, mu[j], r[j]);
+      fast_chunk<CH>(h, lam, mu, r, (double)n, mn, mx);
+    } else {
+      for (int j = 0; j < cnt; j++) {
+        double mu, r; tab.load(n + j, mu, r);
+        h.p = step_div(h.p, lam, d_mul(lam, r), mu, r, mn, mx);
+        h.sum = d_add(h.sum, h.p);
+        h.T = d_fma((double)(n + j + 1), h.p, h.T);
+        h.A = d_add(h.A, d_min(d_mul(h.sum, 0x1p-53), h.p));
+      }
+    }
+    states += live ? cnt : 0;
+    const int n0 = n;
+    n += cnt;
+    // a lane that leaves keeps running with lambda = 0: its terms are 0 and its accumulators stay as they are
+    const bool oob = live & ((mn < WVA_HI_LO) | (mx >= WVA_HI_HI));
+    const bool leave = live & !oob & (n < NH) & fast_head_exit(m, lam, mu0, n0, n, h.p, h.sum);
+    h.ok = h.ok & !oob;
+    if (leave) { h.exited = true; h.n = n; p_exit = h.p; }
+    if (oob | leave) { live = false; lam = 0.0; }
+  }
+  if (h.exited) h.p = p_exit;
+  else h.n = n;
+  const bool cert = active && fast_solve_finish(m, lambda, h, st);
+  const bool redo = active && !cert;
+  bool bad = false;
+  if (__any_sync(full, redo)) {
+    SolveStats st2;
+    int sv = 0;
+    lockstep_solve(m, tab, lambda, redo, st2, sv, bad);
+    if (redo) { st = st2; states += sv; atomicAdd(fallbacks, 1ull); }
+  }
+  return bad ? -1 - states : states;
 }
 
 // evaluation values of a finished solve (EvalTTFT / EvalITL, queueanalyzer.go:283-308)

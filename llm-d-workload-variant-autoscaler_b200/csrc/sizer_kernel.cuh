@@ -21,6 +21,7 @@ struct SizerCounters {
   int pad_;
   unsigned long long lockstep_slots; // lock-step lane sizer: 32 x (longest chain of the warp), summed over rounds
                                      // (states / lockstep_slots = share of the lane-steps that did live work)
+  unsigned long long certify_fallbacks; // pool sizer: fast solves (E12) not certified, redone by the exact solver
 };
 
 // Largest max-batch-size N any pair that needs sizing will use (allocation.go:79-88):

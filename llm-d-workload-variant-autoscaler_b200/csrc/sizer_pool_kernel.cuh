@@ -7,7 +7,7 @@
 //   * a CTA keeps a pool of P pairs whose state (the SizerLane of wva_core.cuh) and head-table rows live in global
 //     memory (L2-resident: ~1.4 KB per pair at N = 256);
 //   * every solve a pair still needs is a REQUEST — the pair's slot — queued in shared memory by length class
-//     (32 log-spaced classes of the estimate N + 37.4 / -ln(lambda / mu_N), capped at K);
+//     (32 log-spaced classes of the solve's cost; with the certified fast solve (E12) that is the head length N);
 //   * a warp takes 32 requests from the fullest class (filling up from its neighbours), loads the 32 pairs' models,
 //     solves them in lock step, advances each pair's bisection / Size / Analyze state machine (sizer_on_solve, the same
 //     code as every other sizer), stores the state back and queues the pair's next request — or retires the pair and
@@ -81,15 +81,12 @@ __device__ __forceinline__ float pool_load_model(PoolModel& pm, const PoolEntry*
   return __ldcg(reinterpret_cast<const float*>(reinterpret_cast<const char*>(e) + offsetof(SizerLane, cur_x)));
 }
 
-// length class of the solve at arrival rate x: the early exit (E4) leaves the chain ~37.4 / -ln(x / mu_N) states after
-// the head, so chains of one class differ by < 2^(1/4) in length
+// length class of the solve at arrival rate x: the certified fast solve (E12) visits at most the N - 1 head states
+// whatever the rate (the tail is closed-form), so the class is that of N; pairs of one N land in one class and their
+// batches take the uniform-N path
 __device__ __forceinline__ int pool_class(const PairModel& m, float x) {
-  float ratio = x / (float)m.mu_last;
-  if (!(ratio > 1e-6f)) ratio = 1e-6f;
-  if (ratio > 0.999999f) ratio = 0.999999f;
-  float est = (float)m.N + 37.4f / -__logf(ratio);
-  const float K = (float)m.K;
-  if (est > K) est = K;
+  (void)x;
+  const float est = (float)m.N;
   int c = (int)(__log2f(fmaxf(est, 32.0f) * (1.0f / 32.0f)) * 4.0f);
   return c < 0 ? 0 : (c >= POOL_NCLS ? POOL_NCLS - 1 : c);
 }
@@ -252,7 +249,9 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
     if (uniform) {
       if (!live) { pm.m.N = nref; pm.m.K = nref + nref * WVA_QUEUE_TO_BATCH; pm.m.mono = 0; pm.m.mu_last = 1.0; pm.m.r_last = 1.0; }
       TileTable tt; tt.rows = rows; tt.row_stride = row_stride; tt.slot = live ? my_slot : 0; tt.tile = tile; tt.n_head = nref - 1;
-      lockstep_solve(pm.m, tt, x, live, st, sv, bad);
+      sv = lockstep_solve_fast(pm.m, tt, x, live, st, &ctr->certify_fallbacks);
+      bad = sv < 0;
+      if (bad) sv = -1 - sv;
     }
     if (live) {
       PoolEntry ze;

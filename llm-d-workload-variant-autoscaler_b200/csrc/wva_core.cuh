@@ -27,6 +27,10 @@
 //        any accumulator (adding t to s with s + t == s, all later t' <= t).
 //   (E5) p[] is not stored: pass 1 finds sum, pass 2 recomputes the recurrence and
 //        accumulates on the normalised p[i] exactly like the reference (quirk Q4).
+//   (E12) only float32 statistics leave a solve: a solve may take its float64 values from
+//        one head pass and a closed-form tail (fast_solve_finish) when an error enclosure
+//        of the reference's float64 values proves that their float32 roundings are the
+//        reference's; otherwise the lane is re-solved by the exact solver.
 #pragma once
 #include <stdint.h>
 #include <math.h>
@@ -350,6 +354,171 @@ WVA_HD void literal_solve(const PairModel& m, float lambda, double* p, SolveStat
   st.avgServTime = f_div(st.avgNumInServers, st.throughput);
   float w = f_sub(st.avgRespTime, st.avgServTime);
   st.avgWaitTime = (w < 0.0f) ? 0.0f : w;
+}
+
+// ------------------------------------------------------------------ (E12) certified fast solve
+// The reference evaluates ~3K roundings per solve, but its consumers only read three float32 values:
+// (float)Lserv, (float)L and f_sub(1, (float)p[K]).  The fast solve runs ONE pass over the head (n < N-1, the same
+// E1 step as the exact solver, so p~[0..N-1] and their sequential sum are the reference's bits), then forms the tail
+// n >= N-1, where mu is the constant mu_last and p~[N-1+k] = p~[N-1] rho^k, in closed form.  It also bounds
+//   (a) the distance of the reference's float64 values from the exact real values, and
+//   (b) the distance of its own values from the exact real values,
+// and accepts a lane only if every float32 value the consumers read is the same at both ends of
+// [v - 4(a+b), v + 4(a+b)] (the factor 4 covers second-order terms and the rounding of the bound itself).
+// Proof sketch (DESIGN.md §3, E12).  u = 2^-53; all terms are non-negative.  Write p_n for the exact chain,
+// S = sum p_n, T = sum n p_n, L = T/S, and R = the rounding error of a sequential sum of non-negative terms:
+// adding t to s errs by at most min(u (s+t), t).
+//   (a) reference: p~_n = p_n (1+th), |th| <= 2n u; its sum errs by <= 2u T + sum_n min(u S, p~_n) =: 2u T + Aref with
+//       Aref <= A_head + u T + A_tail, where A_head accumulates min(u * partial sum, p~_n) in the head pass (the partial
+//       sum falls short of S by the remaining mass; summed over n that is <= T) and A_tail = min(M u S, S_tail).  Hence
+//       the normalising sum has relative error eta <= 2u L + Aref/S + u, and
+//         L:      |L_ref - L|  <= L ((3K + 2) u + eta)                 (i^2 p_i <= K i p_i; K accumulations)
+//         Lserv:  Lserv_ref = L_N + (1 - sumP_N) N; the N-weighted error of sumP_N gives the absolute term:
+//                 |Ls_ref - Ls| <= Ls ((5N + 4) u + eta) + N (eta + 3u + Aref/S)
+//         p[K]:   |pK_ref - pK| <= pK ((2K + 1) u + eta) + 2^-1000     (underflowed terms: K 2^-1074 each, at most)
+//   (b) fast path: running error analysis of the closed form below (first order; every quantity carries its bound).
+//       rho^M by binary powering is within (M - 1) u of rho_hat^M and rho_hat = RN(lambda/mu) is conditioned M times
+//       through the power: 2M u relative, plus 2^-1000 absolute for underflow (all factors <= 1).
+//       1 - rho = (mu - lambda)/mu is formed without cancellation (mu - lambda of two float32 values is exact).
+// Preconditions (otherwise not certified): every head x = p~*lambda inside the E3 window, p~[N-1] and S inside it,
+// N >= 2 and 1 - rho >= 2^-12.  The last one keeps rho < 1 (the closed form needs a convergent tail) with margin;
+// rates the sizer and the grid evaluate stay below lambda_max = 0.999 mu_{N-1}, so it never rejects an admitted rate.
+// Light loads leave the head early (fast_head_exit) once lambda <= mu_n/2 on the whole rest of the chain: the
+// remainder is then below a geometric series of ratio 1/2, sum_{j>n} p~_j <= p~_n and sum_{j>n} j p~_j <= (n+2) p~_n,
+// and those bounds are added to the error of every value.
+#ifndef WVA_TILE_CHUNK
+#define WVA_TILE_CHUNK 16
+#endif
+#define WVA_FAST_OMEGA_MIN 0x1p-12
+
+struct FastHead {  // what the head pass leaves for fast_solve_finish
+  double p;        // p~[n] of the last state visited
+  double sum;      // sequential sum of p~[0..n] (the reference's partial sum, bit for bit)
+  double T;        // sum of j p~[j], j <= n (fma accumulation)
+  double A;        // sum of min(2^-53 * partial sum, p~[j]): the reference's rounding error of the head sum
+  int n;           // index of the last state visited (N - 1 unless the pass left early)
+  bool ok;         // every x = p~ lambda of the pass was inside the exponent window
+  bool exited;     // left the head early (light load): the rest of the chain is the bounded remainder
+};
+
+WVA_HD double d_min(double a, double b) { return a < b ? a : b; }
+
+// chunk-boundary early exit of the head pass; mu0 = mu at the chunk's first state n0 (mu is non-decreasing from
+// n0 >= mono on, the tail rate included), p = p~[n], sum = partial sum at n
+WVA_HD bool fast_head_exit(const PairModel& m, double lam, double mu0, int n0, int n, double p, double sum) {
+  return n0 >= m.mono && d_mul(lam, 2.0) <= mu0 && d_mul(p, (double)(n + 2 + m.N)) <= d_mul(sum, 0x1p-64);
+}
+
+// does v +- r round to one float32 (and to what)?
+WVA_HD bool f32_certain(double v, double r) { return (float)d_sub(v, r) == (float)d_add(v, r); }
+
+// closed-form tail, error enclosure and certification.  true: st holds the reference's statistics
+WVA_HD bool fast_solve_finish(const PairModel& m, float lambda, const FastHead& h, SolveStats& st) {
+  const double u = 0x1p-53, tiny = 0x1p-1000;
+  const int N = m.N, K = m.K;
+  if (!h.ok || N < 2 || !(h.T > 0.0)) return false;
+  const double hn = (double)h.n;
+  // head, against exact arithmetic: sum errs by 2u T + A (recurrence, accumulation), T by 3 n u T (and fma)
+  const double eH = d_add(d_mul(d_mul(2.0, u), h.T), h.A), eTH = d_mul(d_mul(d_mul(3.0, hn), u), h.T);
+  double S, T, num, pKn, eS, eT, eN, epKn, Atail;
+  if (h.exited) {
+    const double RS = h.p, RT = d_mul(h.p, hn + 2.0);     // remainder bounds (ratio <= 1/2 from n on)
+    S = h.sum; T = h.T; num = h.T; pKn = 0.0;
+    eS = d_add(eH, RS); eT = d_add(eTH, RT); eN = d_add(eTH, d_add(RT, d_mul((double)N, RS))); epKn = RS;
+    Atail = RS;
+  } else {
+    const double q = h.p;
+    if (!in_window(q)) return false;
+    const double lam = (double)lambda, mu = m.mu_last;
+    const double om = d_div(d_sub(mu, lam), mu);          // 1 - rho, rel. error <= 2u
+    if (!(om >= WVA_FAST_OMEGA_MIN)) return false;
+    const double rho = d_div(lam, mu);                     // rel. error <= u
+    const int M = K - N + 1;                               // tail states N .. K: p~[N-1+k] = q rho^k, k = 1..M
+    const double dM = (double)M;
+    double a = 1.0, b = rho;                               // a = rho^M
+    for (int e = M; e; e >>= 1) { if (e & 1) a = d_mul(a, b); b = d_mul(b, b); }
+    const double ea = d_add(d_mul(a, d_mul(d_mul(2.0, dM), u)), tiny);              // absolute
+    const double c1 = d_sub(1.0, a), ec1 = d_add(ea, d_mul(u, c1));                 // 1 - rho^M, absolute
+    if (!(c1 > 0.0)) return false;
+    const double G1 = d_div(d_mul(rho, c1), om);                                    // sum rho^k
+    const double rG1 = d_add(d_div(ec1, c1), d_mul(5.0, u));                        // relative
+    const double bM = d_mul(d_mul(dM, a), rho);                                     // M rho^(M+1)
+    const double ebM = d_add(d_mul(bM, d_mul(3.0, u)), d_mul(dM, ea));
+    const double dd = d_sub(G1, bM);
+    if (!(dd > 0.0)) return false;
+    const double G2 = d_div(dd, om);                                                // sum k rho^k
+    const double rG2 = d_add(d_div(d_add(d_add(d_mul(G1, rG1), ebM), d_mul(u, dd)), dd), d_mul(3.0, u));
+    const double rq = d_mul(d_mul(2.0, hn), u);                                     // p~[N-1] vs exact
+    const double St = d_mul(q, G1), rSt = d_add(d_add(rq, rG1), u);
+    const double in = d_add(d_mul(hn, G1), G2);
+    const double rin = d_add(d_add(rG1, u) > rG2 ? d_add(rG1, u) : rG2, u);
+    const double Tt = d_mul(q, in), rTt = d_add(d_add(rq, rin), u);
+    S = d_add(h.sum, St);
+    if (!in_window(S)) return false;
+    T = d_add(h.T, Tt);
+    num = d_add(h.T, d_mul((double)N, St));                // Lserv = (T_head + N S_tail) / S
+    pKn = d_mul(q, a);                                      // p~[K]
+    eS = d_add(d_add(eH, d_mul(St, rSt)), d_mul(u, S));
+    eT = d_add(d_add(eTH, d_mul(Tt, rTt)), d_mul(u, T));
+    eN = d_add(d_add(eTH, d_mul(d_mul((double)N, St), d_add(rSt, u))), d_mul(u, num));
+    epKn = d_add(d_mul(q, ea), d_mul(pKn, d_add(rq, u)));
+    Atail = d_min(d_mul(d_mul(dM, u), S), St);
+  }
+  const double L = d_div(T, S), Ls = d_div(num, S), pK = d_div(pKn, S);
+  const double rS = d_div(eS, S);
+  // (b) fast values against exact arithmetic
+  const double eL = d_mul(L, d_add(d_add(d_div(eT, T), rS), u));
+  const double eLs = d_mul(Ls, d_add(d_add(d_div(eN, num), rS), u));
+  const double epK = d_add(d_div(epKn, S), d_mul(pK, d_add(rS, u)));
+  // (a) the reference against exact arithmetic
+  const double Aref = d_add(d_add(h.A, d_mul(u, T)), Atail), rA = d_div(Aref, S);
+  const double eta = d_add(d_add(d_mul(d_mul(2.0, u), L), rA), u);
+  const double fL = d_mul(L, d_add(d_mul((double)(3 * K + 2), u), eta));
+  const double fLs = d_add(d_mul(Ls, d_add(d_mul((double)(5 * N + 4), u), eta)),
+                           d_mul((double)N, d_add(d_add(eta, d_mul(3.0, u)), rA)));
+  const double fpK = d_add(d_mul(pK, d_add(d_mul((double)(2 * K + 1), u), eta)), tiny);
+  const double radL = d_mul(4.0, d_add(eL, fL)), radLs = d_mul(4.0, d_add(eLs, fLs)), radpK = d_mul(4.0, d_add(epK, fpK));
+  if (!f32_certain(L, radL) || !f32_certain(Ls, radLs)) return false;
+  const double pK_hi = d_add(pK, radpK);
+  if (!(pK_hi < 0x1p-26) && f_sub(1.0f, (float)d_sub(pK, radpK)) != f_sub(1.0f, (float)pK_hi)) return false;
+  st.avgNumInServers = (float)Ls;
+  st.avgNumInSystem = (float)L;
+  st.throughput = f_mul(lambda, f_sub(1.0f, (float)pK));
+  st.avgRespTime = f_div(st.avgNumInSystem, st.throughput);
+  st.avgServTime = f_div(st.avgNumInServers, st.throughput);
+  float w = f_sub(st.avgRespTime, st.avgServTime);
+  st.avgWaitTime = (w < 0.0f) ? 0.0f : w;
+  return true;
+}
+
+// One fast solve on a single lane (the host replay of lockstep_solve_fast; the device runs the same steps, chunks
+// and exit tests with the table prefetched into shared memory).  Returns whether it is certified.
+WVA_HD bool fast_solve(const PairModel& m, float lambda, SolveStats& st, int* states) {
+  FastHead h;
+  h.p = 1.0; h.sum = 1.0; h.T = 0.0; h.A = 0.0; h.n = 0; h.ok = true; h.exited = false;
+  const double lam = (double)lambda;
+  const int NH = m.N - 1;
+  int n = 0;
+  while (n < NH) {
+    const int cnt = NH - n < WVA_TILE_CHUNK ? NH - n : WVA_TILE_CHUNK;
+    const double mu0 = (double)m.tab[(size_t)n * m.stride];
+    for (int j = 0; j < cnt; j++) {
+      const float m32 = m.tab[(size_t)(n + j) * m.stride];
+      const double mu = (double)m32, r = rcp_f32den(m32, mu);
+      const double x = d_mul(h.p, lam);
+      if (!in_window(x)) h.ok = false;
+      h.p = div_f32den(x, mu, r);
+      h.sum = d_add(h.sum, h.p);
+      h.T = d_fma((double)(n + j + 1), h.p, h.T);
+      h.A = d_add(h.A, d_min(d_mul(h.sum, 0x1p-53), h.p));
+    }
+    n += cnt;
+    if (!h.ok) break;
+    if (n < NH && fast_head_exit(m, lam, mu0, n - cnt, n, h.p, h.sum)) { h.exited = true; break; }
+  }
+  h.n = n;
+  *states = n;
+  return fast_solve_finish(m, lambda, h, st);
 }
 
 // utils.go:12-23
