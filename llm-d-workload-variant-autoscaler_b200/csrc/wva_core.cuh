@@ -376,10 +376,13 @@ WVA_HD void literal_solve(const PairModel& m, float lambda, double* p, SolveStat
 //         Lserv:  Lserv_ref = L_N + (1 - sumP_N) N; the N-weighted error of sumP_N gives the absolute term:
 //                 |Ls_ref - Ls| <= Ls ((5N + 4) u + eta) + N (eta + 3u + Aref/S)
 //         p[K]:   |pK_ref - pK| <= pK ((2K + 1) u + eta) + 2^-1000     (underflowed terms: K 2^-1074 each, at most)
+//                 evaluated at the upper end pK + epK of (b): after a head exit the fast p[K] is 0 and only epK bounds it
 //   (b) fast path: running error analysis of the closed form below (first order; every quantity carries its bound).
 //       rho^M by binary powering is within (M - 1) u of rho_hat^M and rho_hat = RN(lambda/mu) is conditioned M times
 //       through the power: 2M u relative, plus 2^-1000 absolute for underflow (all factors <= 1).
 //       1 - rho = (mu - lambda)/mu is formed without cancellation (mu - lambda of two float32 values is exact).
+//       p[K] = q rho^M / S carries 2^-1000 absolute of its own: q rho^M and the quotient may be subnormal (1 ulp =
+//       2^-1074 each), and the 2^-1000 inside the error of rho^M is scaled by q / S <= 1, so it can underflow with them.
 // Preconditions (otherwise not certified): every head x = p~*lambda inside the E3 window, p~[N-1] and S inside it,
 // N >= 2 and 1 - rho >= 2^-12.  The last one keeps rho < 1 (the closed form needs a convergent tail) with margin;
 // rates the sizer and the grid evaluate stay below lambda_max = 0.999 mu_{N-1}, so it never rejects an admitted rate.
@@ -390,6 +393,12 @@ WVA_HD void literal_solve(const PairModel& m, float lambda, double* p, SolveStat
 #define WVA_TILE_CHUNK 16
 #endif
 #define WVA_FAST_OMEGA_MIN 0x1p-12
+// Test hook: fast_solve_finish hands its values (L, Lserv, p[K]), their bounds (b) eL, eLs, epK and (a) fL, fLs, fpK and
+// whether the head pass left early to WVA_FAST_PROBE right before certification.  Empty in the product; the host tests
+// define it to check every bound against exact arithmetic.
+#ifndef WVA_FAST_PROBE
+#define WVA_FAST_PROBE(...)
+#endif
 
 struct FastHead {  // what the head pass leaves for fast_solve_finish
   double p;        // p~[n] of the last state visited
@@ -469,15 +478,16 @@ WVA_HD bool fast_solve_finish(const PairModel& m, float lambda, const FastHead& 
   // (b) fast values against exact arithmetic
   const double eL = d_mul(L, d_add(d_add(d_div(eT, T), rS), u));
   const double eLs = d_mul(Ls, d_add(d_add(d_div(eN, num), rS), u));
-  const double epK = d_add(d_div(epKn, S), d_mul(pK, d_add(rS, u)));
+  const double epK = d_add(d_add(d_div(epKn, S), d_mul(pK, d_add(rS, u))), tiny);
   // (a) the reference against exact arithmetic
   const double Aref = d_add(d_add(h.A, d_mul(u, T)), Atail), rA = d_div(Aref, S);
   const double eta = d_add(d_add(d_mul(d_mul(2.0, u), L), rA), u);
   const double fL = d_mul(L, d_add(d_mul((double)(3 * K + 2), u), eta));
   const double fLs = d_add(d_mul(Ls, d_add(d_mul((double)(5 * N + 4), u), eta)),
                            d_mul((double)N, d_add(d_add(eta, d_mul(3.0, u)), rA)));
-  const double fpK = d_add(d_mul(pK, d_add(d_mul((double)(2 * K + 1), u), eta)), tiny);
+  const double fpK = d_add(d_mul(d_add(pK, epK), d_add(d_mul((double)(2 * K + 1), u), eta)), tiny);
   const double radL = d_mul(4.0, d_add(eL, fL)), radLs = d_mul(4.0, d_add(eLs, fLs)), radpK = d_mul(4.0, d_add(epK, fpK));
+  WVA_FAST_PROBE(L, Ls, pK, eL, fL, eLs, fLs, epK, fpK, h.exited);
   if (!f32_certain(L, radL) || !f32_certain(Ls, radLs)) return false;
   const double pK_hi = d_add(pK, radpK);
   if (!(pK_hi < 0x1p-26) && f_sub(1.0f, (float)d_sub(pK, radpK)) != f_sub(1.0f, (float)pK_hi)) return false;
