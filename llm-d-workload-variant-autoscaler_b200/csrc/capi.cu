@@ -436,6 +436,19 @@ int32_t wva_set_option(wva_ctx* ctx, int32_t option, int32_t value) {
   return WVA_ERR_ARG;
 }
 
+#ifdef WVA_POOL_PHASES
+/* profiling build only (tools/perf_pool_phases.py): copies the pool sizer's phase sums out (out != NULL) and clears them */
+int32_t wva_pool_phases(wva_ctx* ctx, uint64_t* out) {
+  if (!ctx) return WVA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaDeviceSynchronize());
+  if (out) CK(cudaMemcpyFromSymbol(out, g_pool_phase, sizeof(g_pool_phase)));
+  static const unsigned long long zero[PH_N] = {};
+  CK(cudaMemcpyToSymbol(g_pool_phase, zero, sizeof(zero)));
+  return WVA_OK;
+}
+#endif
+
 int32_t wva_calculate(wva_ctx* ctx) {
   if (!ctx) return WVA_ERR_ARG;
   if (!ctx->loaded) { ctx->last_error = "wva_calculate before wva_load_system"; return WVA_ERR_STATE; }

@@ -485,14 +485,12 @@ __device__ __forceinline__ void fast_chunk(FastHead& h, double lam, const double
   h.p = pn[CH]; h.sum = sm[CH];
 }
 
-// One solve per lane at `lambda` (inactive lanes ride along): the fast head pass for every active lane, the closed-form
-// tail and certification (fast_solve_finish), then the exact lockstep_solve for the lanes that were not certified.
-// Returns the states visited (the fallback's included), or -1 - states when the solve is `bad` as for lockstep_solve (by
-// value: out-parameters cost the callers stack and spills).  Every lane that takes the exact solver adds 1 to *fallbacks
-// (rare: a counter in registers would be live across the caller's whole loop).
+// One solve per lane at `lambda` (inactive lanes ride along): the fast head pass for every active lane, then the
+// closed-form tail and certification (fast_solve_finish).  Sets `cert` where st holds the reference's statistics and
+// returns the head states visited.
 template <class Tab>
-__device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& tab, float lambda, bool active, SolveStats& st,
-                                                unsigned long long* fallbacks) {
+__device__ __forceinline__ int lockstep_fast_head(const PairModel& m, const Tab& tab, float lambda, bool active,
+                                                  SolveStats& st, bool& cert) {
   constexpr int CH = Tab::kChunk;
   static_assert(CH == WVA_TILE_CHUNK, "the head pass exits at the chunk boundaries the host replay (fast_solve) uses");
   const unsigned full = 0xffffffffu;
@@ -534,7 +532,20 @@ __device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& t
   }
   if (h.exited) h.p = p_exit;
   else h.n = n;
-  const bool cert = active && fast_solve_finish(m, lambda, h, st);
+  cert = active && fast_solve_finish(m, lambda, h, st);
+  return states;
+}
+
+// The fast solve, then the exact lockstep_solve for the lanes that were not certified (in the same batch: for callers
+// whose fallbacks are too rare to queue).  Returns the states visited (the fallback's included), or -1 - states when the
+// solve is `bad` as for lockstep_solve (by value: out-parameters cost the callers stack and spills).  Every lane that
+// takes the exact solver adds 1 to *fallbacks (rare: a counter in registers would be live across the caller's whole loop).
+template <class Tab>
+__device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& tab, float lambda, bool active, SolveStats& st,
+                                                unsigned long long* fallbacks) {
+  const unsigned full = 0xffffffffu;
+  bool cert;
+  int states = lockstep_fast_head(m, tab, lambda, active, st, cert);
   const bool redo = active && !cert;
   bool bad = false;
   if (__any_sync(full, redo)) {
@@ -544,6 +555,16 @@ __device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& t
     if (redo) { st = st2; states += sv; atomicAdd(fallbacks, 1ull); }
   }
   return bad ? -1 - states : states;
+}
+
+// The fast solve alone, for callers that queue the lanes it does not certify for an exact batch of their own: returns
+// the head states visited, or -1 - states when the lane's solve is not certified.
+template <class Tab>
+__device__ __noinline__ int lockstep_solve_fast_only(const PairModel& m, const Tab& tab, float lambda, bool active,
+                                                     SolveStats& st) {
+  bool cert;
+  const int states = lockstep_fast_head(m, tab, lambda, active, st, cert);
+  return cert || !active ? states : -1 - states;
 }
 
 // evaluation values of a finished solve (EvalTTFT / EvalITL, queueanalyzer.go:283-308)
