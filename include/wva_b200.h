@@ -161,7 +161,7 @@ typedef struct wva_timing {
   float d2h_ms;
   int64_t chain_solves;    /* chain solves executed by the last calculate/grid    */
   int64_t chain_states;    /* birth-death states visited by the last calculate/grid */
-  int64_t overflow_pairs;  /* pairs that took the float64 overflow-rescale slow path  */
+  int64_t overflow_pairs;  /* float64 overflow-rescale slow path: pairs (calculate), levels (grid) */
   float exchange_ms;       /* NCCL exchange of the last wva_solve / wva_saturation_run on a ctx with a communicator
                               (all-gather of the candidate arena or of the solution, all-reduce of the partials) */
   int32_t sizer_kernel;    /* which sizer the last wva_calculate ran: 1 warp per pair, 2 lane per pair (head table in
@@ -283,6 +283,10 @@ int32_t wva_get_solution(wva_ctx* ctx, wva_solution* out);
  * frontier [S*A]: smallest r whose metrics meet every non-zero SLO of the server
  *   (ttft <= slo_ttft, itl <= slo_itl), 0 if none in 1..R — the per-(model,
  *   variant) feasible frontier the north-star design reduces to.
+ * Levels whose chain overflows float64 get the reference's rescaled metrics like
+ * every other level (timing overflow_pairs counts them); more than
+ * min(S*A*R, 16*S*A + 1024) of them in one run is WVA_ERR_LIMIT.  Batch sizes
+ * above 10188 are WVA_ERR_LIMIT.
  */
 int32_t wva_analyze_grid(wva_ctx* ctx, int32_t R, uint8_t* ok, float* ttft,
                          float* itl, float* rho, float* tput, int32_t* frontier);

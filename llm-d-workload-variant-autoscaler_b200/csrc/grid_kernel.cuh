@@ -27,7 +27,38 @@ struct GridCounters {
   unsigned long long slots0, slots_rest, rounds;   // 32 x longest chain of the round: first round of a pair / later rounds
   unsigned long long slots_def;                   // the same for the deferred pass
   unsigned long long certify_fallbacks;           // deferred pass: fast solves (E12) redone by the exact solver
+  unsigned long long pathological;                // overflow pass: literal solves whose rescale loop the reference never leaves
 };
+
+// Levels whose chain overflows float64 (CH_OVERFLOW).  The reference's Analyze still returns metrics for them
+// (computeProbabilities rescales, mm1modelstatedependent.go:84-89,96-104), which needs every earlier p[i]: both passes
+// append the level's output index pair * R + r - 1 here, and grid_overflow_kernel solves them with literal_solve.
+// ctr->overflow counts every level; only the first `cap` are stored, and the host fails the run if any is missing.
+struct GridOverflowList {
+  unsigned long long* items;
+  unsigned long long cap;
+};
+__device__ __forceinline__ void grid_overflow_push(const GridOverflowList& ol, GridCounters* ctr, unsigned long long o) {
+  const unsigned long long k = atomicAdd(&ctr->overflow, 1ull);
+  if (k < ol.cap) ol.items[k] = o;
+}
+
+// Analyze's outputs for one admitted level (queueanalyzer.go:143-166; ttft as allocation.go:148); true if the level meets
+// every SLO of its server
+__device__ __forceinline__ bool grid_store(const GridOut& out, size_t o, const PairModel& m, const SolveStats& st, float lambda,
+                                           float slo_ttft, float slo_itl, float slo_tps, float lambda_tps) {
+  float pf, dec, avg_ttft;
+  eval_values(m, st, &avg_ttft, &dec, &pf);
+  float rho = f_div(st.avgNumInServers, (float)m.N);
+  rho = fminf(fmaxf(rho, 0.0f), 1.0f);
+  if (out.ok) out.ok[o] = 1;
+  if (out.ttft) out.ttft[o] = f_add(st.avgWaitTime, pf);
+  if (out.itl) out.itl[o] = dec;
+  if (out.rho) out.rho[o] = rho;
+  if (out.tput) out.tput[o] = f_mul(st.throughput, 1000.0f);
+  return (slo_ttft <= 0.0f || avg_ttft <= slo_ttft) && (slo_itl <= 0.0f || dec <= slo_itl) &&
+         (slo_tps <= 0.0f || lambda <= lambda_tps);
+}
 
 // Deferral of the near-saturation levels (large systems).  A pair's chain length is a steep function of lambda / mu_N
 // (early exit E4): the one or two lowest admitted levels of a pair run thousands of states next to ~50 for the rest, so a
@@ -81,7 +112,8 @@ __device__ __forceinline__ bool grid_setup(PairModel& m, const SysView& s, int s
 
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, WARPS == 8 ? 2 : 1)
-grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax, GridCounters* ctr, GridDefer df) {
+grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax, GridCounters* ctr, GridDefer df,
+            GridOverflowList ol) {
   extern __shared__ double2 smem_grid[];
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -166,23 +198,25 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
             unsigned long long base = 0;
             if (lane == 0) base = atomicAdd(df.n_items, (unsigned long long)__popc(wm));
             base = __shfl_sync(full, base, 0);
-            if (base + __popc(wm) <= df.cap) {              // room in the list: these levels leave the warp
-              defer[c] = want;
-              if (want) {
-                const unsigned long long k = base + __popc(wm & ((1u << lane) - 1u));
-                df.items[k] = (pair << 16) | (unsigned long long)r[c];
-                df.cls[k] = (unsigned char)grid_class(m, ratio);
-              }
-              if (!saved) {
-                saved = true;
-                float* row = df.rows + (size_t)pair * df.row_stride;
-                for (int n = lane; n < m.N; n += 32) row[n] = tabf[n];
-                if (lane == 0) {
-                  GridSide sd;
-                  sd.m = m; sd.m.tab = row; sd.m.stride = 1;
-                  sd.total_rate = total_rate; sd.slo_ttft = slo_ttft; sd.slo_itl = slo_itl; sd.slo_tps = slo_tps; sd.lambda_tps = lambda_tps;
-                  df.side[pair] = sd;
-                }
+            // the first `room` wanting lanes (by ballot rank) take the slots left in the list and leave the warp; the rest
+            // are solved here.  So every slot below min(n_items, cap) is written exactly once.
+            const unsigned long long room = base < df.cap ? df.cap - base : 0ull;
+            const unsigned rank = __popc(wm & ((1u << lane) - 1u));
+            defer[c] = want && rank < room;
+            if (defer[c]) {
+              const unsigned long long k = base + rank;
+              df.items[k] = (pair << 16) | (unsigned long long)r[c];
+              df.cls[k] = (unsigned char)grid_class(m, ratio);
+            }
+            if (room > 0 && !saved) {                       // warp-uniform: the first level of the pair that leaves
+              saved = true;
+              float* row = df.rows + (size_t)pair * df.row_stride;
+              for (int n = lane; n < m.N; n += 32) row[n] = tabf[n];
+              if (lane == 0) {
+                GridSide sd;
+                sd.m = m; sd.m.tab = row; sd.m.stride = 1;
+                sd.total_rate = total_rate; sd.slo_ttft = slo_ttft; sd.slo_itl = slo_itl; sd.slo_tps = slo_tps; sd.lambda_tps = lambda_tps;
+                df.side[pair] = sd;
               }
             }
           }
@@ -202,7 +236,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
       }
       if (bad) {
         // a chain of this lane left the exponent window: redo its levels one by one through the per-lane state machine
-        // (IEEE divisions); a true float64 overflow stays flagged (only the sizer has the rescale path)
+        // (IEEE divisions); a true float64 overflow goes to the overflow list
 #pragma unroll
         for (int c = 0; c < 2; c++)
           if (here[c]) {
@@ -211,40 +245,28 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
             ch.tail_ok = d_bits(ch.lamg) <= d_bits(m.mu_last);
             while (!chain_step(ch, m, st[c])) {}
             ovf[c] = ch.phase == CH_OVERFLOW;
-            if (ovf[c]) atomicAdd(&ctr->overflow, 1ull);
+            if (ovf[c]) grid_overflow_push(ol, ctr, obase + (size_t)(r[c] - 1));
           }
       }
 #pragma unroll
       for (int c = 0; c < 2; c++) {
-        if (in_range[c] && !defer[c]) {
+        if (in_range[c] && !defer[c] && !ovf[c]) {
           const size_t o = obase + (size_t)(r[c] - 1);
-          if (!admitted[c] || ovf[c]) {
+          if (!admitted[c]) {
             if (out.ok) out.ok[o] = 0;
             if (out.ttft) out.ttft[o] = 0.0f;
             if (out.itl) out.itl[o] = 0.0f;
             if (out.rho) out.rho[o] = 0.0f;
             if (out.tput) out.tput[o] = 0.0f;
-          } else {
-            // Analyze: queueanalyzer.go:143-166
-            float pf, dec, avg_ttft;
-            eval_values(m, st[c], &avg_ttft, &dec, &pf);
-            float rho = f_div(st[c].avgNumInServers, (float)m.N);
-            rho = fminf(fmaxf(rho, 0.0f), 1.0f);
-            if (out.ok) out.ok[o] = 1;
-            if (out.ttft) out.ttft[o] = f_add(st[c].avgWaitTime, pf);   // allocation.go:148
-            if (out.itl) out.itl[o] = dec;
-            if (out.rho) out.rho[o] = rho;
-            if (out.tput) out.tput[o] = f_mul(st[c].throughput, 1000.0f);
-            const bool meets = (slo_ttft <= 0.0f || avg_ttft <= slo_ttft) && (slo_itl <= 0.0f || dec <= slo_itl) &&
-                               (slo_tps <= 0.0f || lambda[c] <= lambda_tps);
-            if (meets && r[c] < front) front = r[c];
+          } else if (grid_store(out, o, m, st[c], lambda[c], slo_ttft, slo_itl, slo_tps, lambda_tps) && r[c] < front) {
+            front = r[c];
           }
         }
       }
     }
     for (int o = 16; o; o >>= 1) front = min(front, __shfl_down_sync(full, front, o));
-    // with deferral the deferred pass still lowers the frontier (atomicMin); grid_frontier_fix maps "none" to 0
-    if (out.frontier && lane == 0) out.frontier[pair] = deferring ? front : ((front == 0x7fffffff) ? 0 : front);
+    // the deferred and overflow passes may still lower the frontier (atomicMin); grid_frontier_fix maps "none" to 0
+    if (out.frontier && lane == 0) out.frontier[pair] = front;
     __syncwarp();
   }
   for (int o = 16; o; o >>= 1) {
@@ -260,7 +282,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
 // The deferred levels, sorted by length class: lane per (pair, level), 32 different pairs per warp.
 __global__ void __launch_bounds__(256, 2)
 grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long* __restrict__ items, unsigned long long n_items,
-                     GridCounters* ctr, unsigned long long* next_item) {
+                     GridCounters* ctr, unsigned long long* next_item, GridOverflowList ol) {
   extern __shared__ __align__(16) float grid_tiles[];
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -307,28 +329,10 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
     }
     if (live) {
       my_solves++; my_states += (unsigned long long)sv;
-      if (ovf) atomicAdd(&ctr->overflow, 1ull);
       const size_t o = (size_t)pair * (size_t)R + (size_t)(r - 1);
-      if (ovf) {
-        if (out.ok) out.ok[o] = 0;
-        if (out.ttft) out.ttft[o] = 0.0f;
-        if (out.itl) out.itl[o] = 0.0f;
-        if (out.rho) out.rho[o] = 0.0f;
-        if (out.tput) out.tput[o] = 0.0f;
-      } else {
-        float pf, dec, avg_ttft;
-        eval_values(m, st, &avg_ttft, &dec, &pf);
-        float rho = f_div(st.avgNumInServers, (float)m.N);
-        rho = fminf(fmaxf(rho, 0.0f), 1.0f);
-        if (out.ok) out.ok[o] = 1;
-        if (out.ttft) out.ttft[o] = f_add(st.avgWaitTime, pf);
-        if (out.itl) out.itl[o] = dec;
-        if (out.rho) out.rho[o] = rho;
-        if (out.tput) out.tput[o] = f_mul(st.throughput, 1000.0f);
-        const bool meets = (slo_ttft <= 0.0f || avg_ttft <= slo_ttft) && (slo_itl <= 0.0f || dec <= slo_itl) &&
-                           (slo_tps <= 0.0f || lambda <= lambda_tps);
-        if (meets && out.frontier) atomicMin(&out.frontier[pair], r);
-      }
+      if (ovf) grid_overflow_push(ol, ctr, o);
+      else if (grid_store(out, o, m, st, lambda, slo_ttft, slo_itl, slo_tps, lambda_tps) && out.frontier)
+        atomicMin(&out.frontier[pair], r);
     }
     {
       int mxs = live ? sv : 0;
@@ -344,6 +348,34 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
     atomicAdd(&ctr->solves, my_solves); atomicAdd(&ctr->states, my_states);
     atomicAdd(&ctr->slots_def, my_slots); atomicAdd(&ctr->rounds, my_rounds);
   }
+}
+
+// The overflow list, one thread per level: the pair's model is rebuilt from the system into a per-thread table, the
+// level is solved by the literal stored-p[] algorithm with the reference's rescale branches (p holds K + 1 doubles),
+// and its outputs are written as above.
+__global__ void __launch_bounds__(64) grid_overflow_kernel(SysView s, int R, GridOut out, const unsigned long long* items,
+                                                           int n, int nmax, double* pbuf, float* tabbuf, GridCounters* ctr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long o = items[i];
+  const unsigned long long pair = o / (unsigned)R;
+  const int r = (int)(o % (unsigned)R) + 1;
+  const int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
+  PairModel m;
+  float total_rate = 0, slo_ttft = 0, slo_itl = 0, slo_tps = 0;
+  int lim = 0;
+  if (!grid_setup(m, s, srv, acc, nmax, &total_rate, &slo_ttft, &slo_itl, &slo_tps, &lim)) return;   // listed levels pass it
+  float* tab = tabbuf + (size_t)i * nmax;
+  double* p = pbuf + (size_t)i * ((size_t)nmax * (WVA_QUEUE_TO_BATCH + 1) + 1);
+  model_fill_table(m, tab, 1, 0, 1);
+  model_finish(m, tab, 1);
+  const float lambda_tps = f_mul(m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));
+  const float lambda = f_div(f_div(total_rate, (float)r), 1000.0f);
+  SolveStats st;
+  bool patho = false;
+  literal_solve(m, lambda, p, st, &patho);
+  if (patho) atomicAdd(&ctr->pathological, 1ull);
+  if (grid_store(out, o, m, st, lambda, slo_ttft, slo_itl, slo_tps, lambda_tps) && out.frontier) atomicMin(&out.frontier[pair], r);
 }
 
 __global__ void __launch_bounds__(256) grid_frontier_fix_kernel(int* frontier, unsigned long long n) {

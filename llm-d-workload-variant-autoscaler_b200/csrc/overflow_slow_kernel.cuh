@@ -32,6 +32,29 @@ __global__ void __launch_bounds__(64) overflow_slow_kernel(SysView s, CandView o
   if (bad) atomicAdd(patho, 1);
 }
 
+// Scratch for n literal solves of batch size <= nmax — p[0..K] (K + 1 doubles) and an N-entry float32 head table per
+// item, item i at pbuf + i * (nmax * (WVA_QUEUE_TO_BATCH + 1) + 1) and tabbuf + i * nmax — handed out at most 1 GiB at a
+// time: launch(first item, items, pbuf, tabbuf) enqueues one batch on `stream`.  0 on success.
+template <class Launch>
+static inline int32_t literal_scratch_batches(int n, int nmax, cudaStream_t stream, Launch launch) {
+  const size_t p_len = (size_t)nmax * (WVA_QUEUE_TO_BATCH + 1) + 1;
+  const size_t per_item = p_len * 8 + (size_t)nmax * 4;
+  size_t batch = (size_t)(1ull << 30) / per_item;   // <= 1 GiB of scratch at a time
+  if (batch < 1) batch = 1;
+  if (batch > (size_t)n) batch = (size_t)n;
+  double* pbuf = nullptr; float* tabbuf = nullptr;
+  if (cudaMalloc(&pbuf, batch * p_len * 8) != cudaSuccess) return 1;
+  if (cudaMalloc(&tabbuf, batch * (size_t)nmax * 4) != cudaSuccess) { cudaFree(pbuf); return 1; }
+  int32_t rc = 0;
+  for (size_t off = 0; off < (size_t)n; off += batch) {
+    int cnt = (int)((size_t)n - off < batch ? (size_t)n - off : batch);
+    launch((int)off, cnt, pbuf, tabbuf);
+    if (cudaStreamSynchronize(stream) != cudaSuccess) { rc = 1; break; }
+  }
+  cudaFree(pbuf); cudaFree(tabbuf);
+  return rc;
+}
+
 static inline int32_t run_overflow_slow_path(const SysView& s, const CandView& out, const int* d_list, int n,
                                              cudaStream_t stream, long long* launches) {
   // worst case N is not known here: re-derive it on the host side through a device reduction
@@ -47,21 +70,11 @@ static inline int32_t run_overflow_slow_path(const SysView& s, const CandView& o
   cudaStreamSynchronize(stream);
   if (nmax_h < 1) nmax_h = 1;
   if (nmax_h > 65536) nmax_h = 65536;
-  const size_t per_pair = ((size_t)nmax_h * (WVA_QUEUE_TO_BATCH + 1) + 1) * 8 + (size_t)nmax_h * 4;
-  size_t batch = (size_t)(1ull << 30) / per_pair;   // <= 1 GiB of scratch at a time
-  if (batch < 1) batch = 1;
-  if (batch > (size_t)n) batch = (size_t)n;
-  double* pbuf = nullptr; float* tabbuf = nullptr;
-  if (cudaMalloc(&pbuf, batch * ((size_t)nmax_h * (WVA_QUEUE_TO_BATCH + 1) + 1) * 8) != cudaSuccess) { cudaFree(d_nmax); return 1; }
-  if (cudaMalloc(&tabbuf, batch * (size_t)nmax_h * 4) != cudaSuccess) { cudaFree(pbuf); cudaFree(d_nmax); return 1; }
-  int32_t rc = 0;
-  for (size_t off = 0; off < (size_t)n; off += batch) {
-    int cnt = (int)((size_t)n - off < batch ? (size_t)n - off : batch);
+  int32_t rc = literal_scratch_batches(n, nmax_h, stream, [&](int off, int cnt, double* pbuf, float* tabbuf) {
     overflow_slow_kernel<<<(cnt + 63) / 64, 64, 0, stream>>>(s, out, d_list + off, cnt, nmax_h, pbuf, tabbuf, d_nmax + 1);
     (*launches)++;
-    if (cudaStreamSynchronize(stream) != cudaSuccess) { rc = 1; break; }
-  }
-  cudaFree(pbuf); cudaFree(tabbuf); cudaFree(d_nmax);
+  });
+  cudaFree(d_nmax);
   return rc;
 }
 

@@ -461,7 +461,10 @@ def test_greedy_zero_capacity(pkg, engine, oracle):
 
 
 # ---- replica grid ------------------------------------------------------------------------------------
-@pytest.mark.parametrize("S,A,N,R,stream", [(10, 4, 32, 32, 1), (24, 8, 128, 128, 2), (6, 3, 256, 70, 3)])
+@pytest.mark.parametrize("S,A,N,R,stream", [(10, 4, 32, 32, 1), (24, 8, 128, 128, 2), (6, 3, 256, 70, 3),
+                                            # both sides of every grid_kernel<8|4|1> launch switch, and the largest N
+                                            (12, 3, 1, 40, 4), (12, 3, 2, 40, 5), (5, 3, 409, 33, 6), (5, 3, 410, 33, 7),
+                                            (3, 2, 2547, 16, 8), (3, 2, 2548, 16, 9), (2, 2, 10188, 8, 10)])
 def test_grid_matches_oracle(pkg, engine, oracle, S, A, N, R, stream):
     sysd = pkg.synth.queue_system(S, A, N, stream=stream, R=R)
     engine.load_system(sysd)
@@ -477,7 +480,9 @@ def test_grid_matches_oracle(pkg, engine, oracle, S, A, N, R, stream):
     assert np.array_equal(engine.grid_fetch_frontier(), o["frontier"])
 
 
-@pytest.mark.parametrize("N,R", [(32, 64), (256, 256)])
+@pytest.mark.parametrize("N,R", [(32, 64), (256, 256),
+                                 # one level, and one level either side of a round of 32 / 64 levels
+                                 (32, 1), (32, 31), (32, 33), (64, 63), (64, 65)])
 def test_grid_deferred_levels_match_oracle(pkg, engine, oracle, N, R):
     """WVA_OPT_GRID_DEFER = 2: the near-saturation levels of every pair leave the pair's warp and are solved in a pass
     sorted by chain length (grid_deferred_kernel, TileTable over per-pair rows); every output and the frontier stay
