@@ -24,10 +24,15 @@ namespace wva {
 #define WVA_HI_HI 0x5F300000   // high word of 2^500
 
 // head-table accessors -----------------------------------------------------------------------------
+// Every table also loads a whole chunk of CH states starting at n (load_chunk; n a multiple of CH).
 struct WarpTable {   // one table per warp in shared memory: (mu_n, ~1/mu_n) as float64 pairs, broadcast reads
   static constexpr int kChunk = 16;
   const double2* t;
   __device__ __forceinline__ void load(int n, double& mu, double& r) const { double2 v = t[n]; mu = v.x; r = v.y; }
+  template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
+#pragma unroll
+    for (int j = 0; j < CH; j++) load(n + j, mu[j], r[j]);
+  }
   __device__ __forceinline__ double mu_at(int n) const { return t[n].x; }
   __device__ __forceinline__ void prepare(int) const {}
 };
@@ -38,24 +43,30 @@ struct LaneTable {   // one float32 column per lane ([n][thread], bank = lane); 
   __device__ __forceinline__ void load(int n, double& mu, double& r) const {
     float m32 = t[(size_t)n * stride]; mu = (double)m32; r = rcp_f32den(m32, mu);
   }
+  template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
+#pragma unroll
+    for (int j = 0; j < CH; j++) load(n + j, mu[j], r[j]);
+  }
   __device__ __forceinline__ double mu_at(int n) const { return (double)t[(size_t)n * stride]; }
   __device__ __forceinline__ void prepare(int) const {}
 };
 // Rows in global memory, one per pool slot, and any 32 of them solved together (sizer_pool_kernel.cuh): the warp keeps
 // two shared tiles of 32 head states x 32 lanes ([state][lane], padded: conflict-free).  Tile k+1 is fetched with
 // cp.async (row by row: each row a coalesced 128-byte access, no registers, no scoreboard) while the lanes work on
-// tile k, so the only exposed latency is the first tile of a pass.
+// tile k, so the only exposed latency is the first tile of a pass.  The tile is held as a shared-space address and
+// read with ld.shared (a generic pointer would be read with generic loads), and the table is passed by value, so that
+// a __noinline__ solver keeps its fields in registers.
 struct TileTable {
   static constexpr int kChunk = WVA_TILE_CHUNK;   // states per unrolled chunk of the solver (code size vs loop overhead)
+  static_assert(32 % kChunk == 0, "a chunk lies inside one tile");
   const float* rows;      // base of the CTA's rows
   int row_stride;         // floats per row (a multiple of 32, >= N)
   int slot;               // this lane's row (any valid row for an idle lane)
-  float* tile;            // the warp's two [32][33] tiles in shared memory
+  unsigned tile;          // shared-space address of the warp's two [32][33] tiles
   int n_head;             // head entries (N - 1): tiles beyond are never fetched
   __device__ __forceinline__ void fetch(int n0) const {
     const int lane = threadIdx.x & 31;
-    float* t = tile + ((n0 >> 5) & 1) * (32 * 33);
-    const unsigned dst0 = (unsigned)__cvta_generic_to_shared(t + lane * 33);
+    const unsigned dst0 = tile + 4u * (((n0 >> 5) & 1) * (32 * 33) + lane * 33);
 #pragma unroll 8
     for (int r = 0; r < 32; r++) {
       const int sr = __shfl_sync(0xffffffffu, slot, r);
@@ -63,6 +74,16 @@ struct TileTable {
       asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst0 + 4u * r), "l"(src) : "memory");
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
+  }
+  // shared address of this lane's entry of state n
+  __device__ __forceinline__ unsigned addr(int n) const {
+    return tile + 4u * (((n >> 5) & 1) * (32 * 33) + (n & 31) * 33 + (threadIdx.x & 31));
+  }
+  // volatile: kept after the cp.async wait and __syncwarp of prepare()
+  static __device__ __forceinline__ float lds(unsigned a) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
+    return v;
   }
   __device__ __forceinline__ void prepare(int n) const {
     if (n & 31) return;
@@ -81,11 +102,15 @@ struct TileTable {
     __syncwarp();
   }
   __device__ __forceinline__ void load(int n, double& mu, double& r) const {
-    float m32 = tile[((n >> 5) & 1) * (32 * 33) + (n & 31) * 33 + (threadIdx.x & 31)]; mu = (double)m32; r = rcp_f32den(m32, mu);
+    float m32 = lds(addr(n)); mu = (double)m32; r = rcp_f32den(m32, mu);
   }
-  __device__ __forceinline__ double mu_at(int n) const {
-    return (double)tile[((n >> 5) & 1) * (32 * 33) + (n & 31) * 33 + (threadIdx.x & 31)];
+  // state n + j sits j rows of 33 floats below state n: one address per chunk, immediate offsets after it
+  template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
+    const unsigned a = addr(n);
+#pragma unroll
+    for (int j = 0; j < CH; j++) { float m32 = lds(a + 4u * 33u * j); mu[j] = (double)m32; r[j] = rcp_f32den(m32, mu[j]); }
   }
+  __device__ __forceinline__ double mu_at(int n) const { return (double)lds(addr(n)); }
 };
 
 // high word of v * 2^-54 for a normal v >= 2^-900: the exponent field moves, nothing rounds
@@ -255,15 +280,16 @@ __device__ __forceinline__ void lockstep_solve_inl(const PairModel& m, const Tab
   while (n < NH && !all_done) {                       // head: table entries n .. n+cnt-1
     const int cnt = min(CH, NH - n);
     tab.prepare(n);
-    const double mu0 = tab.mu_at(n);
+    double mu0;
 #pragma unroll
     for (int c = 0; c < NC; c++) { a[c].mn = 0x7fffffff; a[c].mx = 0; }
     if (cnt == CH) {
       double mu[CH], r[CH];
-#pragma unroll
-      for (int j = 0; j < CH; j++) tab.load(n + j, mu[j], r[j]);
+      tab.template load_chunk<CH>(n, mu, r);
+      mu0 = mu[0];
       p1_chunk<NC, CH, true>(a, lam, lamr_l, mu, r);
     } else {
+      mu0 = tab.mu_at(n);
       for (int j = 0; j < cnt; j++) {
         double mu, r; tab.load(n + j, mu, r);
 #pragma unroll
@@ -336,15 +362,16 @@ __device__ __forceinline__ void lockstep_solve_inl(const PairModel& m, const Tab
   while (n < NH && !all_done) {                       // head (i = n+1 <= N-1)
     const int cnt = min(CH, NH - n);
     tab.prepare(n);
-    const double mu0 = tab.mu_at(n);
+    double mu0;
 #pragma unroll
     for (int c = 0; c < NC; c++) { b[c].mn = 0x7fffffff; b[c].mx = 0; }
     if (cnt == CH) {
       double mu[CH], r[CH];
-#pragma unroll
-      for (int j = 0; j < CH; j++) tab.load(n + j, mu[j], r[j]);
+      tab.template load_chunk<CH>(n, mu, r);
+      mu0 = mu[0];
       p2_chunk<NC, CH, true>(b, lam, lamr_l, mu, r, sum, rsum, di);
     } else {
+      mu0 = tab.mu_at(n);
       for (int j = 0; j < cnt; j++) {
         double mu, r; tab.load(n + j, mu, r);
         di = d_add(di, 1.0);
@@ -442,13 +469,13 @@ __device__ __forceinline__ void lockstep_solve_inl(const PairModel& m, const Tab
 }
 
 template <int NC, class Tab>
-__device__ __noinline__ void lockstep_solve_n(const PairModel& m, const Tab& tab, const float* lambda,
+__device__ __noinline__ void lockstep_solve_n(const PairModel& m, const Tab tab, const float* lambda,
                                               const bool* active, SolveStats* st, int& states, bool& bad) {
   lockstep_solve_inl<NC, Tab>(m, tab, lambda, active, st, states, bad);
 }
 
 template <class Tab>
-__device__ __forceinline__ void lockstep_solve(const PairModel& m, const Tab& tab, float lambda, bool active,
+__device__ __forceinline__ void lockstep_solve(const PairModel& m, const Tab tab, float lambda, bool active,
                                                SolveStats& st, int& states, bool& bad) {
   lockstep_solve_n<1, Tab>(m, tab, &lambda, &active, &st, states, bad);
 }
@@ -485,12 +512,22 @@ __device__ __forceinline__ void fast_chunk(FastHead& h, double lam, const double
   h.p = pn[CH]; h.sum = sm[CH];
 }
 
+// Phase profile of the fast solve (tools/perf_pool_phases.py): built with -DWVA_POOL_PHASES, lockstep_solve_fast_only
+// adds lane 0's clock64() cycles of the first tile wait, the head chunks (the later tile waits included) and
+// fast_solve_finish to ph[0..2].  The product build compiles none of it.
+#ifdef WVA_POOL_PHASES
+#define FAST_PH(...) __VA_ARGS__
+#else
+#define FAST_PH(...)
+#endif
+struct FastPhases { long long wait0, chunks, finish; };
+
 // One solve per lane at `lambda` (inactive lanes ride along): the fast head pass for every active lane, then the
 // closed-form tail and certification (fast_solve_finish).  Sets `cert` where st holds the reference's statistics and
 // returns the head states visited.
 template <class Tab>
-__device__ __forceinline__ int lockstep_fast_head(const PairModel& m, const Tab& tab, float lambda, bool active,
-                                                  SolveStats& st, bool& cert) {
+__device__ __forceinline__ int lockstep_fast_head(const PairModel& m, const Tab tab, float lambda, bool active,
+                                                  SolveStats& st, bool& cert, FastPhases& ph) {
   constexpr int CH = Tab::kChunk;
   static_assert(CH == WVA_TILE_CHUNK, "the head pass exits at the chunk boundaries the host replay (fast_solve) uses");
   const unsigned full = 0xffffffffu;
@@ -501,17 +538,21 @@ __device__ __forceinline__ int lockstep_fast_head(const PairModel& m, const Tab&
   bool live = active;
   int states = 0, n = 0;
   double p_exit = 0.0;
+  FAST_PH(const long long ph_t0 = clock64();)
   while (n < NH && __any_sync(full, live)) {
     const int cnt = min(CH, NH - n);
+    FAST_PH(const long long ph_w = clock64();)
     tab.prepare(n);
-    const double mu0 = tab.mu_at(n);
+    FAST_PH(if (n == 0) ph.wait0 += clock64() - ph_w;)
+    double mu0;
     int mn = 0x7fffffff, mx = 0;
     if (cnt == CH) {
       double mu[CH], r[CH];
-#pragma unroll
-      for (int j = 0; j < CH; j++) tab.load(n + j, mu[j], r[j]);
+      tab.template load_chunk<CH>(n, mu, r);
+      mu0 = mu[0];
       fast_chunk<CH>(h, lam, mu, r, (double)n, mn, mx);
     } else {
+      mu0 = tab.mu_at(n);
       for (int j = 0; j < cnt; j++) {
         double mu, r; tab.load(n + j, mu, r);
         h.p = step_div(h.p, lam, d_mul(lam, r), mu, r, mn, mx);
@@ -532,7 +573,9 @@ __device__ __forceinline__ int lockstep_fast_head(const PairModel& m, const Tab&
   }
   if (h.exited) h.p = p_exit;
   else h.n = n;
+  FAST_PH(const long long ph_t1 = clock64(); ph.chunks += ph_t1 - ph_t0;)
   cert = active && fast_solve_finish(m, lambda, h, st);
+  FAST_PH(__syncwarp(); ph.finish += clock64() - ph_t1;)
   return states;
 }
 
@@ -541,11 +584,12 @@ __device__ __forceinline__ int lockstep_fast_head(const PairModel& m, const Tab&
 // solve is `bad` as for lockstep_solve (by value: out-parameters cost the callers stack and spills).  Every lane that
 // takes the exact solver adds 1 to *fallbacks (rare: a counter in registers would be live across the caller's whole loop).
 template <class Tab>
-__device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& tab, float lambda, bool active, SolveStats& st,
+__device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab tab, float lambda, bool active, SolveStats& st,
                                                 unsigned long long* fallbacks) {
   const unsigned full = 0xffffffffu;
   bool cert;
-  int states = lockstep_fast_head(m, tab, lambda, active, st, cert);
+  FastPhases ph{};
+  int states = lockstep_fast_head(m, tab, lambda, active, st, cert, ph);
   const bool redo = active && !cert;
   bool bad = false;
   if (__any_sync(full, redo)) {
@@ -560,10 +604,12 @@ __device__ __noinline__ int lockstep_solve_fast(const PairModel& m, const Tab& t
 // The fast solve alone, for callers that queue the lanes it does not certify for an exact batch of their own: returns
 // the head states visited, or -1 - states when the lane's solve is not certified.
 template <class Tab>
-__device__ __noinline__ int lockstep_solve_fast_only(const PairModel& m, const Tab& tab, float lambda, bool active,
-                                                     SolveStats& st) {
+__device__ __noinline__ int lockstep_solve_fast_only(const PairModel& m, const Tab tab, float lambda, bool active,
+                                                     SolveStats& st FAST_PH(, unsigned long long* ph_out)) {
   bool cert;
-  const int states = lockstep_fast_head(m, tab, lambda, active, st, cert);
+  FastPhases ph{};
+  const int states = lockstep_fast_head(m, tab, lambda, active, st, cert, ph);
+  FAST_PH(if ((threadIdx.x & 31) == 0) { ph_out[0] += ph.wait0; ph_out[1] += ph.chunks; ph_out[2] += ph.finish; })
   return cert || !active ? states : -1 - states;
 }
 

@@ -119,7 +119,10 @@ enum {
   PH_FAST_BATCHES, PH_FAST_STATES, PH_FAST_SLOTS,                 // batches, live lane-steps, 32 x longest solve
   PH_EXACT_BATCHES, PH_EXACT_STATES, PH_EXACT_SLOTS,
   PH_FAST_PARTIAL, PH_EXACT_PARTIAL,                              // batches of fewer than 32 requests
-  PH_ROWS, PH_ITERS, PH_N
+  PH_ROWS, PH_ITERS,
+  PH_MODEL,                                                       // cycles of fast batches: model load (pool_load_model),
+  PH_FAST_WAIT0, PH_FAST_CHUNKS, PH_FAST_FINISH,                  // first tile wait, head chunks, fast_solve_finish
+  PH_N
 };
 __device__ unsigned long long g_pool_phase[PH_N];
 #define POOL_PH(...) __VA_ARGS__
@@ -144,7 +147,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
   const unsigned lt = (1u << lane) - 1u;
   PoolEntry* pool = pool_all + (size_t)blockIdx.x * P;
   float* rows = rows_all + (size_t)blockIdx.x * P * row_stride;
-  float* tile = sm.tiles[warp];
+  const unsigned tile = (unsigned)__cvta_generic_to_shared(sm.tiles[warp]);
 
   for (int i = threadIdx.x; i < P; i += POOL_THREADS) sm.free_list[i] = (unsigned short)(P - 1 - i);
   if (threadIdx.x < POOL_NCLS) { sm.head[threadIdx.x] = 0; sm.tail[threadIdx.x] = 0; }
@@ -322,6 +325,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
     if (live) x = pool_load_model(pm, pool + my_slot);
     const int nref = __shfl_sync(full, pm.m.N, __ffs(live_mask) - 1);
     const bool uniform = __all_sync(full, !live || pm.m.N == nref);
+    POOL_PH(if (!exact) POOL_PH_ADD(PH_MODEL, clock64() - ph_t);)
     bool bad = false, requeue = false;
     int sv = 0;
     SolveStats st;
@@ -331,7 +335,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       if (exact) {
         lockstep_solve(pm.m, tt, x, live, st, sv, bad);
       } else {
-        sv = lockstep_solve_fast_only(pm.m, tt, x, live, st);
+        sv = lockstep_solve_fast_only(pm.m, tt, x, live, st POOL_PH(, &ph_acc[warp][PH_FAST_WAIT0]));
         requeue = live && sv < 0;
         if (sv < 0) sv = -1 - sv;
       }

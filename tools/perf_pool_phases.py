@@ -2,7 +2,10 @@
 
 Builds the library of a source tree (default: this one) with -DWVA_POOL_PHASES into its own directory, runs
 System.Calculate on the pool sizer and prints each phase's share of the warps' clock64() cycles, and the live
-lane-steps of fast and exact batches.  The product library in the tree is neither used nor touched.
+lane-steps of fast and exact batches.  The fast batches are split further into the model load (pool_load_model), the
+first tile wait of each head pass, the head chunks (the later tile waits included) and fast_solve_finish, and the head
+chunks' cycles are given per warp-state (one state index of a batch: 32 lane-steps, live or not) and per live lane-state.
+The product library in the tree is neither used nor touched.
 
 Usage: perf_pool_phases.py [--root TREE] [--out DIR] [--scale S] [--runs R] [--json FILE]
 """
@@ -19,10 +22,13 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = "llm-d-workload-variant-autoscaler_b200"
 NAMES = ["lock", "new_pairs", "fast", "exact", "state", "total", "fast_batches", "fast_states", "fast_slots",
-         "exact_batches", "exact_states", "exact_slots", "fast_partial", "exact_partial", "rows", "iters"]
+         "exact_batches", "exact_states", "exact_slots", "fast_partial", "exact_partial", "rows", "iters",
+         "model", "fast_wait0", "fast_chunks", "fast_finish"]
 PHASES = {"lock": "critical section", "new_pairs": "new-pair setup + BuildModel",
           "fast": "model load + fast head + finish", "exact": "exact solves",
           "state": "state load + sizer_on_solve + store"}
+FAST_PARTS = {"model": "model load", "fast_wait0": "first tile wait", "fast_chunks": "head chunks",
+              "fast_finish": "fast_solve_finish"}
 
 
 def build(tree: str, out: str) -> str:
@@ -79,6 +85,19 @@ def main():
     for k, txt in PHASES.items():
         print(f"  {txt:<40s} {100 * share[k]:6.2f} %")
     print(f"  {'idle (no request to take)':<40s} {100 * share['idle']:6.2f} %")
+    parts = {k: r[k] / tot for k in FAST_PARTS}
+    parts["fast_other"] = share["fast"] - sum(parts.values())
+    res["fast_parts"] = parts
+    print("  of which, fast batches:")
+    for k, txt in FAST_PARTS.items():
+        print(f"    {txt:<38s} {100 * parts[k]:6.2f} %")
+    print(f"    {'rest (call, batch bookkeeping)':<38s} {100 * parts['fast_other']:6.2f} %")
+    warp_states = r["fast_slots"] / 32
+    res["chunk_cycles_per_warp_state"] = r["fast_chunks"] / max(warp_states, 1)
+    res["chunk_cycles_per_live_lane_state"] = r["fast_chunks"] / max(r["fast_states"], 1)
+    print(f"  head chunks: {res['chunk_cycles_per_warp_state']:.1f} cycles per warp-state "
+          f"({warp_states:.3g} warp-states), {res['chunk_cycles_per_live_lane_state']:.2f} per live lane-state; "
+          f"first tile wait {r['fast_wait0'] / max(r['fast_batches'], 1):.0f} cycles per batch")
     for kind in ("fast", "exact"):
         b, st, sl = r[f"{kind}_batches"], r[f"{kind}_states"], r[f"{kind}_slots"]
         print(f"  {kind} batches {b} ({r[kind + '_partial']} with < 32 requests): live lane-steps {st} of {sl} "
