@@ -226,7 +226,9 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
       SolveStats st[2];
       int sv = 0;
       bool bad = false;
-      if (__any_sync(full, here[0] || here[1])) lockstep_solve_inl<2, WarpTable>(m, WarpTable{tab}, lambda, here, st, sv, bad);
+      // a pair with a service rate outside the (E1) divisor range takes the per-lane chain below for every level
+      if (!m.e1_ok) bad = here[0] || here[1];
+      else if (__any_sync(full, here[0] || here[1])) lockstep_solve_inl<2, WarpTable>(m, WarpTable{tab}, lambda, here, st, sv, bad);
       if (here[0] || here[1]) { my_solves += (here[0] ? 1 : 0) + (here[1] ? 1 : 0); my_states += (unsigned long long)sv; }
       {
         int mxs = (here[0] || here[1]) ? sv : 0;
@@ -235,8 +237,8 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
         first_round = false;
       }
       if (bad) {
-        // a chain of this lane left the exponent window: redo its levels one by one through the per-lane state machine
-        // (IEEE divisions); a true float64 overflow goes to the overflow list
+        // a chain of this lane left the exponent window (or the pair needs IEEE divisions): redo its levels one by one
+        // through the per-lane state machine; a true float64 overflow goes to the overflow list
 #pragma unroll
         for (int c = 0; c < 2; c++)
           if (here[c]) {
@@ -304,7 +306,7 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
     const float rate = f_div(total_rate, (float)r);
     const float lambda = f_div(rate, 1000.0f);
     const int nref = __shfl_sync(full, m.N, 0);
-    const bool uniform = __all_sync(full, m.N == nref);
+    const bool uniform = __all_sync(full, m.N == nref && m.e1_ok);   // else the per-lane chain (IEEE divisions)
     SolveStats st;
     int sv = 0;
     bool bad = false, ovf = false;

@@ -121,8 +121,9 @@ struct P2 { double p, L, sumP, pi; int mn, mx; };
 
 // (E1) with a 3-deep dependency chain: the approximation q0 of x/mu = RN(p*lambda)/mu is formed as
 // p * RN(lambda*r) next to x = p*lambda instead of after it.  q0 only has to be within 2^-39.99 of the
-// quotient (it is within ~2^-45.9: r's 2^-46 plus three roundings); the remainder and the final fma use the
-// exact x, so the result is still the correctly rounded RN(x/mu).
+// quotient (it is within ~2^-45.9: r's 2^-46.56 plus three roundings); the remainder and the final fma use the
+// exact x, so the result is still the correctly rounded RN(x/mu).  Only for mu in [2^-126, 2^126] (e1_divisor): the
+// callers never give this solver a pair with another service rate (PairModel::e1_ok).
 __device__ __forceinline__ double step_div(double p, double lam, double lamr, double mu, double r, int& mn, int& mx) {
   double x = d_mul(p, lam);
   double q0 = d_mul(p, lamr);

@@ -109,7 +109,7 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
     }
     // ---- one round: every live lane solves its chain at z.cur_x -------------------------------
     const int nref = __shfl_sync(full, z.m.N, __ffs(live_mask) - 1);
-    const bool uniform = __all_sync(full, !live || z.m.N == nref);
+    const bool uniform = __all_sync(full, !live || (z.m.N == nref && z.m.e1_ok));   // else the per-lane chain
     bool bad = false;
     int sv = 0;
     if (uniform && !live) { z.m.N = nref; z.m.K = nref + nref * WVA_QUEUE_TO_BATCH; }   // idle lanes only keep the loops uniform

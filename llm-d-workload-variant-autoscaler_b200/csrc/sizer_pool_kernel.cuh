@@ -132,6 +132,30 @@ __device__ unsigned long long g_pool_phase[PH_N];
 #define POOL_PH_ADD(k, v) do {} while (0)
 #endif
 
+// A pair with a service rate outside the (E1) divisor range never enters the queues: its lane runs every solve of the
+// pair through the per-lane chain (chain_step: IEEE divisions by such a rate), a float64 overflow to the slow path as
+// below.  Out of line: it is rare, and inlined it costs the batch loop registers.  Returns false (the pair is done).
+__device__ __noinline__ bool pool_pair_on_chain(PoolEntry& ze, const SysView& s, const CandView& out, SizerCounters* ctr,
+                                                int* overflow_list, unsigned long long& my_states) {
+  SizerLane& z = ze.z;
+  SolveStats st;
+  bool live = true;
+  while (live) {
+    while (!chain_step(z.c, z.m, st)) {}
+    if (z.c.phase == CH_OVERFLOW) {
+      const unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
+      if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
+      z.states += z.c.states;
+      lane_fail(z, s, out);
+      live = false;
+    } else {
+      live = sizer_on_solve(z, s, out, st);
+    }
+  }
+  my_states += z.states;
+  return false;
+}
+
 __global__ void __launch_bounds__(POOL_THREADS, 1)
 sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, int P, PoolEntry* pool_all, float* rows_all,
                   int row_stride, SizerCounters* ctr, int* overflow_list) {
@@ -293,6 +317,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
         if (lane == src) { r0 = first; rl = last; mono = desc; }
       }
       bool live = false;
+      __syncwarp();                                    // the rows' entries, written by every lane, are read back below
       if (need_table) {
         PairModel& m = z.m;
         m.tab = rows + (size_t)new_slot * row_stride; m.stride = 1;
@@ -302,9 +327,16 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
         m.lambda_min = f_div(rmin, 1000.0f);                                                         // :189-190
         m.lambda_max = f_div(m.rate_max, 1000.0f);
         m.mono = mono;
+        // every entry an (E1) divisor?  The row is non-decreasing from mono on, so its ends bound it there; read through
+        // L2, where the lanes wrote it (L1 may still hold the slot's previous row)
+        int e1 = e1_divisor(__ldcg(m.tab + mono)) && e1_divisor(rl);
+        for (int n = 0; n < mono; n++) e1 &= (int)e1_divisor(__ldcg(m.tab + n));
+        m.e1_ok = e1;
         m.mu_last = (double)rl;
         m.r_last = rcp_f32den(rl, m.mu_last);
         live = sizer_begin(z, s, out);
+        // a service rate outside the (E1) divisor range: the whole pair here, on the per-lane chain (rare)
+        if (live && !m.e1_ok) live = pool_pair_on_chain(ze, s, out, ctr, overflow_list, my_states);
         if (!live) my_solves += z.solves;
       }
       if (live) { pool_store(pool + new_slot, ze); pushB = new_slot; clsB = pool_class(z.m); }

@@ -23,6 +23,26 @@ namespace wva {
 
 #if defined(__CUDACC__)
 
+// one solve per lane: in lock step from the shared table, or — for a pair with a service rate outside the (E1) divisor
+// range (warp-uniform: one pair per warp) — through the per-lane chain with IEEE divisions (warp_chain_solve)
+__device__ __noinline__ void warp_chain_solve(const PairModel& m, float x, bool act, SolveStats& st, int& states, bool& ovf) {
+  st = SolveStats{};
+  states = 0;
+  ovf = false;
+  if (!act) return;
+  Chain c;
+  chain_start(c, x);
+  c.tail_ok = d_bits(c.lamg) <= d_bits(m.mu_last);
+  while (!chain_step(c, m, st)) {}
+  ovf = c.phase == CH_OVERFLOW;
+  states = c.states;
+}
+__device__ __forceinline__ void warp_solve(const PairModel& m, const double2* tab, float x, bool act, SolveStats& st,
+                                           int& states, bool& ovf) {
+  if (m.e1_ok) lockstep_solve(m, WarpTable{tab}, x, act, st, states, ovf);
+  else warp_chain_solve(m, x, act, st, states, ovf);
+}
+
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
 sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, SizerCounters* ctr, int* overflow_list) {
@@ -85,7 +105,7 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
         if (lane == 0) { x = m.lambda_min; act = true; }
         else if (lane == 1) { x = m.lambda_max; act = true; }
         else if (lane < 2 + 15) { int node = lane - 1; x = spec_node_x(m.lambda_min, m.lambda_max, node, spec_depth_of(node)); act = true; }
-        lockstep_solve(m, WarpTable{tab}, x, act, st, sv_states, ovf); my_states += sv_states;
+        warp_solve(m, tab, x, act, st, sv_states, ovf); my_states += sv_states;
         solves += 17;
         if (__any_sync(full, act && ovf)) ovf_any = true;
         eval_values(m, st, &y_t, &y_i, &pf);
@@ -117,7 +137,7 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
           else { node = lane + 1; mine_is_I = sI.active; act = lane < 31; }
           const Search& mq = mine_is_I ? sI : sT;
           x = act ? spec_node_x(mq.lo, mq.hi, node, spec_depth_of(node)) : 0.0f;
-          lockstep_solve(m, WarpTable{tab}, x, act, st, sv_states, ovf); my_states += sv_states;
+          warp_solve(m, tab, x, act, st, sv_states, ovf); my_states += sv_states;
           solves += both ? 30 : 31;
           if (__any_sync(full, act && ovf)) { ovf_any = true; break; }
           eval_values(m, st, &y_t, &y_i, &pf);
@@ -141,7 +161,7 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       float request_rate = f_mul(lambda, 1000.0f);
       if (!analyze_admits(m, request_rate)) failed = true;
       else {
-        lockstep_solve(m, WarpTable{tab}, f_div(request_rate, 1000.0f), lane == 0, st, sv_states, ovf); my_states += sv_states;
+        warp_solve(m, tab, f_div(request_rate, 1000.0f), lane == 0, st, sv_states, ovf); my_states += sv_states;
         solves++;
         if (__shfl_sync(full, (int)ovf, 0)) ovf_any = true;
         else {
@@ -153,7 +173,7 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
           float rate = f_div(z.total_rate, (float)nr);
           if (!analyze_admits(m, rate)) failed = true;
           else {
-            lockstep_solve(m, WarpTable{tab}, f_div(rate, 1000.0f), lane == 0, st, sv_states, ovf); my_states += sv_states;
+            warp_solve(m, tab, f_div(rate, 1000.0f), lane == 0, st, sv_states, ovf); my_states += sv_states;
             solves++;
             if (__shfl_sync(full, (int)ovf, 0)) ovf_any = true;
             else if (lane == 0) {

@@ -16,10 +16,12 @@
 // performs is performed here with the same operands, order and rounding.  What is
 // changed is only HOW a correctly-rounded result is obtained and WHICH provably
 // no-op operations are skipped:
-//   (E1) x / mu, mu a float32-valued double: q0 = x*r, rem = fma(-q0,mu,x),
+//   (E1) x / mu, mu a float32-valued double in [2^-126, 2^126]: q0 = x*r, rem = fma(-q0,mu,x),
 //        q = fma(rem,r,q0) with r within 2^-40 of 1/mu is the correctly rounded
 //        quotient, because a quotient by a 24-bit divisor is never closer than
 //        2^-25 ulp to a rounding boundary while the perturbation is < 2^-26 ulp.
+//        A pair with any mu_n outside that range (e1_divisor, PairModel::e1_ok) is solved
+//        by the per-lane chain, which divides by such a mu_n with the IEEE division.
 //   (E2) p / sum: two Markstein correction steps with the correctly rounded
 //        reciprocal (__drcp_rn) give the correctly rounded quotient.
 //   (E3) outside the exponent window [2^-500, 2^500) the plain IEEE division is used.
@@ -76,7 +78,12 @@ WVA_HD double d_mul(double a, double b) { return a * b; }
 WVA_HD double d_div(double a, double b) { return a / b; }
 WVA_HD double d_fma(double a, double b, double c) { return fma(a, b, c); }
 WVA_HD double d_rcp(double a) { return 1.0 / a; }
-WVA_HD float f_rcp_approx(float a) { return 1.0f / a; }
+// rcp.approx.ftz: a subnormal input is read as 0 and a subnormal result is returned as 0
+WVA_HD float f_rcp_approx(float a) {
+  if (fabsf(a) < FLT_MIN) a = copysignf(0.0f, a);
+  const float r = 1.0f / a;
+  return fabsf(r) < FLT_MIN ? copysignf(0.0f, r) : r;
+}
 WVA_HD long long d_bits(double a) { long long b; memcpy(&b, &a, 8); return b; }
 WVA_HD int d_hi(double a) { return (int)(d_bits(a) >> 32); }
 #endif
@@ -93,11 +100,25 @@ WVA_HD double div_f32den(double x, double mu, double r) {
   double rem = d_fma(-q0, mu, x);
   return d_fma(rem, r, q0);
 }
-// reciprocal of a float32-valued double to ~2^-46 (one Newton step on the f32 seed)
-WVA_HD double rcp_f32den(float m32, double mu) {
-  double r0 = (double)f_rcp_approx(m32);
+// one Newton step on a float32 seed s of 1/mu
+WVA_HD double rcp_refine(float s, double mu) {
+  double r0 = (double)s;
   double e = d_fma(-mu, r0, 1.0);
   return d_fma(r0, e, r0);
+}
+// reciprocal of a float32-valued double, for mu in [2^-126, 2^126] only (e1_divisor).  There the seed rcp.approx.ftz.f32
+// is within 1 ulp of RN(1/mu) and |1 - mu r| <= 2^-46.56 (H100, every float32 mu: tests/test_device_prims.py).  Outside,
+// 1/mu is not a float32 normal number and the seed flushes: a subnormal mu reads as 0 (seed inf, r = NaN), mu > 2^126
+// has a subnormal 1/mu (seed 0, r = 0), and mu = inf gives r = NaN.
+WVA_HD double rcp_f32den(float m32, double mu) { return rcp_refine(f_rcp_approx(m32), mu); }
+// mu in [2^-126, 2^126]: the divisors (E1) holds for
+WVA_HD bool e1_divisor(float m32) {
+#if defined(__CUDA_ARCH__)
+  const unsigned b = __float_as_uint(m32);
+#else
+  unsigned b; memcpy(&b, &m32, 4);
+#endif
+  return b - 0x00800000u <= 0x7E800000u - 0x00800000u;
 }
 // (E2) correctly rounded x / y with y53 = RN(1/y)
 WVA_HD double div_markstein2(double x, double y, double y53) {
@@ -132,6 +153,7 @@ struct PairModel {
   int N, K;
   float lambda_min, lambda_max;  // Size(): RateRange.Min/1000, RateRange.Max/1000
   float rate_max;                // RateRange.Max (req/s)
+  int e1_ok;                     // every mu_n is an (E1) divisor; else the pair is solved by the per-lane chain (chain_step)
   // head table: mu_n as float32 at tab[n*stride], n in [0,N)
   const float* tab;
   int stride;
@@ -193,6 +215,10 @@ WVA_HD void model_finish(PairModel& m, const float* tab, int stride) {
     nxt = cur;
   }
   m.mono = mono;
+  // mu is non-decreasing on [mono, N-1]: its ends bound it there, only the entries below mono are checked one by one
+  int e1 = e1_divisor(tab[(size_t)mono * stride]) && e1_divisor(rl);
+  for (int n = 0; n < mono; n++) e1 &= (int)e1_divisor(tab[(size_t)n * stride]);
+  m.e1_ok = e1;
   m.mu_last = (double)rl;
   m.r_last = rcp_f32den(rl, m.mu_last);
 }
@@ -247,7 +273,9 @@ WVA_HD double chain_next(const Chain& c, const PairModel& m, bool* exit_ok) {
     mono_ok = c.tail_ok;
   }
   *exit_ok = mono_ok;
-  if (in_window(x)) return div_f32den(x, mu, r);
+  // (E1) only for an E1 divisor: for any other float32 mu the seed flushes and r is 0 or NaN, whose high word fails the
+  // test (integer ops: this loop is FP64-bound)
+  if (in_window(x) && (unsigned)d_hi(r) - 1u < 0x7FEFFFFFu) return div_f32den(x, mu, r);
   return d_div(x, mu);
 }
 
@@ -504,6 +532,8 @@ WVA_HD bool fast_solve_finish(const PairModel& m, float lambda, const FastHead& 
 // One fast solve on a single lane (the host replay of lockstep_solve_fast; the device runs the same steps, chunks
 // and exit tests with the table prefetched into shared memory).  Returns whether it is certified.
 WVA_HD bool fast_solve(const PairModel& m, float lambda, SolveStats& st, int* states) {
+  *states = 0;
+  if (!m.e1_ok) return false;   // the device never gives such a pair to the fast solve
   FastHead h;
   h.p = 1.0; h.sum = 1.0; h.T = 0.0; h.A = 0.0; h.n = 0; h.ok = true; h.exited = false;
   const double lam = (double)lambda;

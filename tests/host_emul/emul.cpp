@@ -383,46 +383,98 @@ int emul_calculate(const wva_system* sys, wva_candidates* out, int64_t* solves, 
   return 0;
 }
 
-// exact-division self-checks against the IEEE operator; returns number of mismatches
-int64_t emul_check_div_f32den(int64_t n, uint64_t seed) {
+}  // extern "C"
+
+// exact-division self-checks against the IEEE operator; return the number of mismatches.
+// (E1) divisor of the checks: every exponent of [2^-126, 2^126] (e1_divisor), all-ones significands and powers of two
+// included, 2^126 itself now and then
+static float e1_test_divisor(uint64_t b, int64_t i) {
+  uint32_t mm = (uint32_t)(b & 0x7FFFFF);
+  const int me = 1 + (int)((b >> 23) % 252);                          // biased exponent 1 .. 252: 2^-126 .. 2^125
+  if ((i & 7) == 0) mm = 0x7FFFFFu;                                   // all-ones significand
+  if ((i & 7) == 1) mm = 0;                                           // power of two
+  uint32_t mb = ((uint32_t)me << 23) | mm;
+  if ((i & 255) == 2) mb = 0x7E800000u;                               // 2^126, the largest E1 divisor
+  float m32; memcpy(&m32, &mb, 4);
+  return m32;
+}
+// the seeds the device can produce: f_rcp_approx(m) is within seed_ulp ulps of RN(1/m) for every E1 divisor
+// (tests/test_device_prims.py), so every seed within that distance is checked; seeds that leave the normal range are
+// left to the device check (the device flushes them)
+template <class Check>
+static bool for_each_seed(float m32, int seed_ulp, Check check) {
+  const float s0 = 1.0f / m32;
+  bool ok = true;
+  for (int k = -seed_ulp; k <= seed_ulp; k++) {
+    float s = s0;
+    for (int j = 0; j < (k < 0 ? -k : k); j++) s = nextafterf(s, k < 0 ? 0.0f : INFINITY);
+    if (!(s >= FLT_MIN && s <= FLT_MAX)) continue;
+    ok = ok && check(rcp_refine(s, (double)m32));
+  }
+  return ok;
+}
+
+extern "C" {
+
+int64_t emul_check_div_f32den(int64_t n, uint64_t seed, int seed_ulp) {
   std::mt19937_64 g(seed);
   int64_t bad = 0;
   for (int64_t i = 0; i < n; i++) {
     uint64_t a = g(), b = g();
-    // random double with exponent in a wide window, random float32 divisor
-    uint64_t xm = a & 0xFFFFFFFFFFFFFull; int xe = 1023 + (int)((a >> 52) % 600) - 300;
+    // random double with exponent in the E3 window, random E1 divisor
+    uint64_t xm = a & 0xFFFFFFFFFFFFFull; int xe = 1023 + (int)((a >> 52) % 1000) - 500;
     uint64_t xb = ((uint64_t)xe << 52) | xm; double x; memcpy(&x, &xb, 8);
-    uint32_t mm = (uint32_t)(b & 0x7FFFFF); int me = 127 + (int)((b >> 23) % 60) - 30;
-    uint32_t mb = ((uint32_t)me << 23) | mm; float m32; memcpy(&m32, &mb, 4);
-    if ((i & 7) == 0) mb |= 0x7FFFFFu, memcpy(&m32, &mb, 4);           // all-ones significand
-    if ((i & 7) == 1) { mb &= ~0x7FFFFFu; memcpy(&m32, &mb, 4); }       // power of two
-    double mu = (double)m32;
-    double r = rcp_f32den(m32, mu);
-    double q = div_f32den(x, mu, r);
-    if (q != x / mu) bad++;
+    const float m32 = e1_test_divisor(b, i);
+    const double mu = (double)m32;
+    if (!e1_divisor(m32) || rcp_f32den(m32, mu) != rcp_refine(1.0f / m32, mu)) { bad++; continue; }
+    if (!for_each_seed(m32, seed_ulp, [&](double r) { return div_f32den(x, mu, r) == x / mu; })) bad++;
   }
   return bad;
 }
 // the 3-deep variant of (E1) used by lockstep_solve.cuh step_div: q0 = p * RN(lambda*r) formed beside x = p*lambda
-int64_t emul_check_step_div(int64_t n, uint64_t seed) {
+int64_t emul_check_step_div(int64_t n, uint64_t seed, int seed_ulp) {
   std::mt19937_64 g(seed);
   int64_t bad = 0;
   for (int64_t i = 0; i < n; i++) {
     uint64_t a = g(), b = g(), c = g();
-    uint64_t pm = a & 0xFFFFFFFFFFFFFull; int pe = 1023 + (int)((a >> 52) % 400) - 200;
-    uint64_t pb = ((uint64_t)pe << 52) | pm; double p; memcpy(&p, &pb, 8);
-    uint32_t mm = (uint32_t)(b & 0x7FFFFF); int me = 127 + (int)((b >> 23) % 40) - 20;
-    uint32_t mb = ((uint32_t)me << 23) | mm; float m32; memcpy(&m32, &mb, 4);
     uint32_t lm = (uint32_t)(c & 0x7FFFFF); int le = 127 + (int)((c >> 23) % 40) - 20;
     uint32_t lb = ((uint32_t)le << 23) | lm; float l32; memcpy(&l32, &lb, 4);
-    if ((i & 7) == 0) { mb |= 0x7FFFFFu; memcpy(&m32, &mb, 4); }
-    double mu = (double)m32, lam = (double)l32;
-    double r = rcp_f32den(m32, mu);
-    double lamr = d_mul(lam, r);
-    double x = d_mul(p, lam), q0 = d_mul(p, lamr);
-    double rem = d_fma(-q0, mu, x);
-    double q = d_fma(rem, r, q0);
-    if (q != x / mu) bad++;
+    const double lam = (double)l32;
+    // p such that x = p lambda lies in the E3 window
+    uint64_t pm = a & 0xFFFFFFFFFFFFFull; int pe = 1023 + (int)((a >> 52) % 960) - 480;
+    uint64_t pb = ((uint64_t)pe << 52) | pm; double p; memcpy(&p, &pb, 8);
+    const float m32 = e1_test_divisor(b, i);
+    const double mu = (double)m32;
+    const double x = d_mul(p, lam);
+    if (!in_window(x)) continue;
+    if (!for_each_seed(m32, seed_ulp, [&](double r) {
+          double lamr = d_mul(lam, r);
+          double q0 = d_mul(p, lamr);
+          double rem = d_fma(-q0, mu, x);
+          return d_fma(rem, r, q0) == x / mu;
+        }))
+      bad++;
+  }
+  return bad;
+}
+// e1_divisor over every float32 bit pattern: true exactly on [2^-126, 2^126]; returns the number of wrong answers
+int64_t emul_check_e1_range() {
+  int64_t bad = 0;
+  for (uint64_t b = 0; b <= 0xFFFFFFFFull; b++) {
+    float m; const uint32_t b32 = (uint32_t)b; memcpy(&m, &b32, 4);
+    const bool want = m >= 0x1p-126f && m <= 0x1p126f;
+    if (e1_divisor(m) != want) bad++;
+  }
+  return bad;
+}
+// the host f_rcp_approx flushes as rcp.approx.ftz.f32 does: subnormal inputs read as 0, subnormal results are 0
+int64_t emul_check_seed_ftz() {
+  int64_t bad = 0;
+  for (uint32_t b = 1; b < 0x7F800000u; b++) {
+    float m; memcpy(&m, &b, 4);
+    const float s = f_rcp_approx(m);
+    const float want = m < FLT_MIN ? INFINITY : (1.0f / m < FLT_MIN ? 0.0f : 1.0f / m);
+    if (memcmp(&s, &want, 4) != 0) bad++;
   }
   return bad;
 }

@@ -151,7 +151,27 @@ int emul_calculate_fast(const wva_system* sys, wva_candidates* out, int64_t* cou
         SolveStats st{};
         int sv = 0;
         counts[0]++;
-        if (fast_solve(z.m, z.c.lambda, st, &sv)) {
+        if (!z.m.e1_ok) {
+          // a service rate outside the (E1) divisor range: the device solves every chain of the pair with the per-lane
+          // chain (IEEE divisions), neither the fast solve nor the lock-step solver
+          while (!chain_step(z.c, z.m, st)) {}
+          if (z.c.phase == CH_OVERFLOW) {
+            counts[2]++;
+            SizerLane y;
+            int lim2 = 0;
+            sizer_setup(y, s, o, srv, acc, 1 << 20, &lim2);
+            model_finish(y.m, tab.data(), 1);
+            std::vector<double> p((size_t)y.m.K + 1);
+            bool bad = false;
+            bool l2 = sizer_begin(y, s, o);
+            while (l2) {
+              literal_solve(y.m, y.cur_x, p.data(), st, &bad);
+              y.c.states = y.m.K + 1;
+              l2 = sizer_on_solve(y, s, o, st);
+            }
+            break;
+          }
+        } else if (fast_solve(z.m, z.c.lambda, st, &sv)) {
           z.c.states = sv;
         } else {
           counts[1]++;
@@ -218,7 +238,7 @@ extern "C" {
 // wva_analyze_grid with deferral at threshold thr (thr <= 0: none): the levels grid_kernel keeps are solved by the
 // exact chain solver, the deferred ones by the fast solve and, where it is not certified, the exact chain solver, as
 // grid_deferred_kernel does for a batch of one N.  Outputs [S, A, R] and frontier [S, A] as wva_analyze_grid.
-// counts: [0] levels solved, [1] deferred levels, [2] deferred levels not certified, [3] overflow
+// counts: [0] levels solved, [1] deferred levels, [2] deferred levels not certified by the fast solve, [3] overflow
 int emul_grid_deferred(const wva_system* sys, int R, float thr, uint8_t* ok, float* ttft, float* itl, float* rho,
                        float* tput, int32_t* frontier, int64_t* counts) {
   SysView s = make_view(sys);
@@ -242,8 +262,8 @@ int emul_grid_deferred(const wva_system* sys, int R, float thr, uint8_t* ok, flo
         counts[0]++;
         SolveStats st{};
         bool solved = false;
-        if (deferred) {
-          counts[1]++;
+        if (deferred) counts[1]++;
+        if (deferred && m.e1_ok) {                     // grid_deferred_kernel: per-lane chain for the other pairs
           int sv = 0;
           solved = fast_solve(m, lambda, st, &sv);
           if (!solved) counts[2]++;

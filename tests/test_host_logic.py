@@ -10,6 +10,9 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# Largest distance, in float32 ulps, of the device's reciprocal seed rcp.approx.ftz.f32 from the correctly rounded 1/mu
+# over the (E1) divisors [2^-126, 2^126]; test_device_prims.py measures it over every float32 on the H100.
+SEED_MAX_ULP = 1
 F32_FIELDS = ("cost", "value", "itl", "ttft", "rho", "max_arrv_rate")
 
 
@@ -21,9 +24,11 @@ def emul(pkg):
     abi = pkg._abi
     lib.emul_calculate.argtypes = [C.POINTER(abi.System), C.POINTER(abi.Candidates)] + [C.POINTER(C.c_int64)] * 3
     lib.emul_check_div_f32den.restype = C.c_int64
-    lib.emul_check_div_f32den.argtypes = [C.c_int64, C.c_uint64]
+    lib.emul_check_div_f32den.argtypes = [C.c_int64, C.c_uint64, C.c_int]
     lib.emul_check_step_div.restype = C.c_int64
-    lib.emul_check_step_div.argtypes = [C.c_int64, C.c_uint64]
+    lib.emul_check_step_div.argtypes = [C.c_int64, C.c_uint64, C.c_int]
+    lib.emul_check_e1_range.restype = C.c_int64
+    lib.emul_check_seed_ftz.restype = C.c_int64
     lib.emul_check_div_markstein2.restype = C.c_int64
     lib.emul_check_div_markstein2.argtypes = [C.c_int64, C.c_uint64]
 
@@ -73,10 +78,19 @@ def _bit_equal(a, b):
 
 
 def test_exact_division_tricks(emul):
-    """(E1)/(E2) of csrc/wva_core.cuh against the IEEE operator, incl. all-ones / power-of-two divisors."""
-    assert emul.emul_check_div_f32den(5_000_000, 1) == 0
+    """(E1)/(E2) of csrc/wva_core.cuh against the IEEE operator, incl. all-ones / power-of-two divisors.  The E1 checks
+    draw divisors from every exponent of [2^-126, 2^126] and refine every seed within SEED_MAX_ULP of RN(1/mu), the
+    seeds the device's rcp.approx.ftz.f32 can return there."""
+    assert emul.emul_check_div_f32den(2_000_000, 1, SEED_MAX_ULP) == 0
     assert emul.emul_check_div_markstein2(5_000_000, 2) == 0
-    assert emul.emul_check_step_div(5_000_000, 3) == 0
+    assert emul.emul_check_step_div(2_000_000, 3, SEED_MAX_ULP) == 0
+
+
+def test_e1_divisor_range_and_host_seed_flush(emul):
+    """e1_divisor is true exactly on [2^-126, 2^126] over all 2^32 float32 bit patterns, and the host seed flushes like
+    rcp.approx.ftz.f32: a subnormal mu reads as 0 (seed inf), a subnormal 1/mu is returned as 0."""
+    assert emul.emul_check_e1_range() == 0
+    assert emul.emul_check_seed_ftz() == 0
 
 
 @pytest.mark.parametrize("S,A,N,stream", [(10, 4, 32, 1), (40, 8, 16, 7), (12, 6, 128, 2), (4, 4, 256, 3),
