@@ -431,14 +431,52 @@ int32_t wva_ingest_write(wva_ingest* ing, int32_t which /* WVA_VEC_* */, int64_t
 /* metric batch -> decisions: one CUDA graph launch (wva_timing.saturation_ms = device time of the whole graph) */
 int32_t wva_ingest_commit(wva_ingest* ing);
 
+/*
+ * Decision mode: the same graph carried on to the cycle's final decisions — the rest of optimizeV1
+ * (internal/engines/saturation/engine.go:322-392) for every model at once, with no host round trip inside:
+ *   Enforcer.EnforcePolicy per model (pipeline/enforcer.go:55-183; targets = var_target, -1 = absent from the map;
+ *   has_cost = the variant has a reporting pod, analyzer.go:148-149, else DefaultVariantCost 10; variants of a model in
+ *   ascending name order) -> convertSaturationTargetsToDecisions (engine.go:589-661) -> DefaultLimiter.Limit over all
+ *   decisions of the cycle (pipeline/default_limiter.go:42-81, the pipeline of wva_limit) when enable_limiter != 0.
+ * A model none of whose pods reported produces no decision and runs no enforcer (prepareModelData returns nil,
+ * engine.go:737-742).  wva_ingest_create_decisions returns the plain `cols` / `res` (filled exactly as by
+ * wva_ingest_create: pre-enforcer targets and analyses) plus the views below; begin / write / commit / destroy are
+ * shared with the plain mode.  Every decision column is per cycle: the graph reads it at each commit.
+ */
+typedef struct wva_ingest_decision_columns {   /* page-locked host memory owned by the wva_ingest; filled every cycle  */
+  int32_t n_types;                   /* T: accelerator types of the inventory                                          */
+  int32_t* var_accelerator_type;     /* [V] index in [0, T) of VariantSaturationAnalysis.AcceleratorName (engine.go:648);
+                                      *     -1 (or any value outside [0, T)) = "" or a type without a pool              */
+  int32_t* var_gpus_per_replica;     /* [V] VariantReplicaState.GPUsPerReplica (<= 0 reads 1, engine.go:624-628)      */
+  uint8_t* mod_scale_to_zero_enabled;/* [M] IsScaleToZeroEnabled for the model (enforcer.go:66)                     */
+  double* mod_request_count;         /* [M] requestCountFunc's count over the retention period (enforcer.go:100,109) */
+  uint8_t* mod_request_error;        /* [M] the request-count query failed: targets kept (enforcer.go:101-105)       */
+  int32_t* type_limit;               /* [T] TypeInventory limitByType after Refresh (default_limiter.go:47-50)       */
+  int32_t* enable_limiter;           /* [1] SaturationScalingConfig.EnableLimiter (engine.go:370); 0 = final = original */
+} wva_ingest_decision_columns;
+typedef struct wva_ingest_decision_results {   /* page-locked host memory owned by the wva_ingest                     */
+  uint8_t* has_decision;             /* [V] a VariantDecision exists: reporting model, enforced target >= 0 (:611)   */
+  int32_t* original_target;          /* [V] OriginalTargetReplicas = the enforced target (:636); -1 without decision */
+  int32_t* target;                   /* [V] TargetReplicas after the limiter (greedy_saturation_algorithm.go:100)     */
+  int32_t* gpus_allocated;           /* [V] GPUsAllocated (greedy_saturation_algorithm.go:99)                         */
+  uint8_t* was_limited;              /* [V] WasLimited (greedy_saturation_algorithm.go:103-105)                       */
+  int8_t* action;                    /* [V] Action before the limiter (:614-622): 1 scale-up, -1 scale-down, 0 no-change */
+  uint8_t* mod_enforcer_applied;     /* [M] EnforcePolicy's second result (engine.go:334-341)                        */
+} wva_ingest_decision_results;
+int32_t wva_ingest_create_decisions(wva_ctx* ctx, int64_t n_models, int64_t n_variants, int64_t n_slots, int32_t n_types,
+                                    const int32_t* model_variant_off /* [M+1] */, const int32_t* variant_slot_off /* [V+1] */,
+                                    wva_ingest** out, wva_ingest_columns* cols, wva_ingest_results* res,
+                                    wva_ingest_decision_columns* dcols, wva_ingest_decision_results* dres);
+
 /* ---- GPU-count limiter ---------------------------------------------------- */
 /*
  * DefaultLimiter.Limit (internal/engines/pipeline/default_limiter.go:42-81) with
  * TypeInventory.CreateAllocator / typeAllocator.TryAllocate
  * (type_inventory.go:222-243,347-373) and GreedyBySaturation.Allocate
  * (greedy_saturation_algorithm.go:34-108).  D decisions, T accelerator types.
- * acc_type[d] = -1 encodes AcceleratorName == "".  Outputs are the mutated
- * VariantDecision fields.
+ * acc_type[d] = -1 (or any value outside [0, T)) encodes AcceleratorName == "".
+ * Outputs are the mutated VariantDecision fields.  Any T >= 0 is supported: the
+ * type pass sorts as many key bits as T + 2 segments need.
  */
 int32_t wva_limit(wva_ctx* ctx, int64_t n_decisions, int32_t n_types,
                   const int32_t* acc_type, const int32_t* current,

@@ -309,4 +309,15 @@ class IngestResults(C.Structure):
                 ("mod_total_replicas", _i32p), ("partials", _i64p)]
 
 
+class IngestDecisionColumns(C.Structure):
+    _fields_ = [("n_types", C.c_int32), ("var_accelerator_type", _i32p), ("var_gpus_per_replica", _i32p),
+                ("mod_scale_to_zero_enabled", _u8p), ("mod_request_count", _f64p), ("mod_request_error", _u8p),
+                ("type_limit", _i32p), ("enable_limiter", _i32p)]
+
+
+class IngestDecisionResults(C.Structure):
+    _fields_ = [("has_decision", _u8p), ("original_target", _i32p), ("target", _i32p), ("gpus_allocated", _i32p),
+                ("was_limited", _u8p), ("action", C.POINTER(C.c_int8)), ("mod_enforcer_applied", _u8p)]
+
+
 VEC_KV_CACHE_USAGE, VEC_QUEUE_LENGTH = 0, 1

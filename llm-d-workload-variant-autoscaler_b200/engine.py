@@ -73,6 +73,9 @@ def load_library():
     L.wva_group_saturation_v1.argtypes = [ctxp, C.POINTER(abi.SaturationIn), C.POINTER(abi.SaturationOut)]
     L.wva_ingest_create.argtypes = [ctxp, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(ctxp),
                                     C.POINTER(abi.IngestColumns), C.POINTER(abi.IngestResults)]
+    L.wva_ingest_create_decisions.argtypes = [ctxp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.POINTER(ctxp), C.POINTER(abi.IngestColumns), C.POINTER(abi.IngestResults),
+                                              C.POINTER(abi.IngestDecisionColumns), C.POINTER(abi.IngestDecisionResults)]
     L.wva_ingest_destroy.argtypes = [ctxp]
     L.wva_ingest_begin.argtypes = [ctxp]
     L.wva_ingest_write.argtypes = [ctxp, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]
@@ -112,7 +115,7 @@ EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_l
            "wva_microbench_fp64", "wva_set_optimizer", "wva_set_capacity", "wva_comm_unique_id", "wva_comm_init_rank",
            "wva_comm_shard", "wva_group_create", "wva_group_destroy", "wva_group_size", "wva_group_ctx",
            "wva_group_optimize", "wva_group_saturation_v1", "wva_ingest_create", "wva_ingest_destroy", "wva_ingest_begin",
-           "wva_ingest_write", "wva_ingest_commit"]
+           "wva_ingest_write", "wva_ingest_commit", "wva_ingest_create_decisions"]
 
 
 def comm_unique_id() -> bytes:
@@ -404,17 +407,29 @@ class Ingest:
     """wva_ingest: the collector's columnar staging + the streaming reconcile as one CUDA graph (include/wva_b200.h).
 
     registry: model_variant_off [M+1], variant_slot_off [V+1] (CSR model -> variant -> pod slot; slots of a variant in
-    ascending pod-name order).  `cols` / `res` are numpy views of the page-locked arenas the library owns."""
+    ascending pod-name order).  `cols` / `res` are numpy views of the page-locked arenas the library owns.
 
-    def __init__(self, engine: "Engine", model_variant_off, variant_slot_off):
+    n_types=None: the plain graph (analysis + pre-enforcer targets).  n_types=T >= 0: the decision mode
+    (wva_ingest_create_decisions) — the same graph carried on through the enforcer, the decisions and the GPU limiter;
+    `dcols` (filled every cycle) and `dres` are then the views of its extra columns and results, and `res` is unchanged."""
+
+    def __init__(self, engine: "Engine", model_variant_off, variant_slot_off, n_types=None):
         self.engine, self.lib = engine, engine.lib
         mvo = np.ascontiguousarray(model_variant_off, np.int32); vso = np.ascontiguousarray(variant_slot_off, np.int32)
         M, V, S = mvo.size - 1, vso.size - 1, int(vso[-1])
         self.M, self.V, self.S = M, V, S
+        self.model_variant_off = mvo
+        self.T = None if n_types is None else int(n_types)
         self.h = C.c_void_p()
         cst, rst = abi.IngestColumns(), abi.IngestResults()
-        engine._check(self.lib.wva_ingest_create(engine.ctx, M, V, S, mvo.ctypes.data, vso.ctypes.data, C.byref(self.h),
-                                                 C.byref(cst), C.byref(rst)), "wva_ingest_create")
+        if self.T is None:
+            engine._check(self.lib.wva_ingest_create(engine.ctx, M, V, S, mvo.ctypes.data, vso.ctypes.data, C.byref(self.h),
+                                                     C.byref(cst), C.byref(rst)), "wva_ingest_create")
+        else:
+            dcst, drst = abi.IngestDecisionColumns(), abi.IngestDecisionResults()
+            engine._check(self.lib.wva_ingest_create_decisions(engine.ctx, M, V, S, self.T, mvo.ctypes.data, vso.ctypes.data,
+                                                               C.byref(self.h), C.byref(cst), C.byref(rst), C.byref(dcst),
+                                                               C.byref(drst)), "wva_ingest_create_decisions")
 
         def view(p, n, dt):
             if n == 0:
@@ -433,6 +448,19 @@ class Ingest:
                     "var_avg_spare_kv": view(rst.var_avg_spare_kv, V, np.float64),
                     "var_avg_spare_queue": view(rst.var_avg_spare_queue, V, np.float64), "mod_flags": view(rst.mod_flags, M, np.uint8),
                     "mod_total_replicas": view(rst.mod_total_replicas, M, np.int32), "partials": view(rst.partials, 4, np.int64)}
+        self.dcols = self.dres = None
+        if self.T is not None:
+            T = self.T
+            self.dcols = {"var_accelerator_type": view(dcst.var_accelerator_type, V, np.int32),
+                          "var_gpus_per_replica": view(dcst.var_gpus_per_replica, V, np.int32),
+                          "mod_scale_to_zero_enabled": view(dcst.mod_scale_to_zero_enabled, M, np.uint8),
+                          "mod_request_count": view(dcst.mod_request_count, M, np.float64),
+                          "mod_request_error": view(dcst.mod_request_error, M, np.uint8),
+                          "type_limit": view(dcst.type_limit, T, np.int32), "enable_limiter": view(dcst.enable_limiter, 1, np.int32)}
+            self.dres = {"has_decision": view(drst.has_decision, V, np.uint8), "original_target": view(drst.original_target, V, np.int32),
+                         "target": view(drst.target, V, np.int32), "gpus_allocated": view(drst.gpus_allocated, V, np.int32),
+                         "was_limited": view(drst.was_limited, V, np.uint8), "action": view(drst.action, V, np.int8),
+                         "mod_enforcer_applied": view(drst.mod_enforcer_applied, M, np.uint8)}
 
     def begin(self):
         self.engine._check(self.lib.wva_ingest_begin(self.h), "wva_ingest_begin")

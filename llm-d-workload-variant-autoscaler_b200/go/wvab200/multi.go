@@ -161,13 +161,27 @@ type Ingest struct {
 	h      *C.wva_ingest
 	cols   C.wva_ingest_columns
 	res    C.wva_ingest_results
+	dcols  C.wva_ingest_decision_columns // decision mode only (NewIngestDecisions)
+	dres   C.wva_ingest_decision_results
 	slotOf map[string]int32 // pod name -> slot
 	kv, q  []float64
 	has    []uint8
+	nv, nm int
 }
 
 // models: sorted model ids; variants[m]: sorted VariantAutoscaling names of model m; pods[variant]: its pod names.
 func NewIngest(ctx *Ctx, models []string, variants map[string][]string, pods map[string][]string) (*Ingest, error) {
+	return newIngest(ctx, models, variants, pods, -1)
+}
+
+// NewIngestDecisions: the same registry in decision mode (wva_ingest_create_decisions) — Commit() then runs the rest of
+// optimizeV1 (engine.go:322-392: EnforcePolicy per model, convertSaturationTargetsToDecisions, the GPU limiter over all
+// decisions) inside the graph.  nTypes = accelerator types of the GPU inventory, in sorted name order.
+func NewIngestDecisions(ctx *Ctx, models []string, variants map[string][]string, pods map[string][]string, nTypes int) (*Ingest, error) {
+	return newIngest(ctx, models, variants, pods, nTypes)
+}
+
+func newIngest(ctx *Ctx, models []string, variants map[string][]string, pods map[string][]string, nTypes int) (*Ingest, error) {
 	ing := &Ingest{slotOf: map[string]int32{}}
 	mvo := []C.int32_t{0}
 	vso := []C.int32_t{0}
@@ -184,11 +198,18 @@ func NewIngest(ctx *Ctx, models []string, variants map[string][]string, pods map
 		}
 		mvo = append(mvo, C.int32_t(nv))
 	}
-	rc := C.wva_ingest_create(ctx.c, C.int64_t(len(models)), C.int64_t(nv), C.int64_t(len(ing.slotOf)), &mvo[0], &vso[0],
-		&ing.h, &ing.cols, &ing.res)
+	var rc C.int32_t
+	if nTypes < 0 {
+		rc = C.wva_ingest_create(ctx.c, C.int64_t(len(models)), C.int64_t(nv), C.int64_t(len(ing.slotOf)), &mvo[0], &vso[0],
+			&ing.h, &ing.cols, &ing.res)
+	} else {
+		rc = C.wva_ingest_create_decisions(ctx.c, C.int64_t(len(models)), C.int64_t(nv), C.int64_t(len(ing.slotOf)),
+			C.int32_t(nTypes), &mvo[0], &vso[0], &ing.h, &ing.cols, &ing.res, &ing.dcols, &ing.dres)
+	}
 	if err := ctx.err(rc, "wva_ingest_create"); err != nil {
 		return nil, err
 	}
+	ing.nv, ing.nm = nv, len(models)
 	n := len(ing.slotOf)
 	ing.kv = unsafe.Slice((*float64)(unsafe.Pointer(ing.cols.kv)), n) // page-locked C memory: cgo pointer rules do not apply
 	ing.q = unsafe.Slice((*float64)(unsafe.Pointer(ing.cols.queue)), n)
@@ -221,4 +242,70 @@ func (g *Ingest) Commit() error {
 		return fmt.Errorf("wva_ingest_commit: %s", C.GoString(C.wva_strerror(rc)))
 	}
 	return nil
+}
+
+// IngestDecisionInputs: the per-cycle columns of the decision mode, indexed like the registry (variants / models) and
+// the inventory's sorted types.  AcceleratorType -1 = "" or a type without a pool.
+type IngestDecisionInputs struct {
+	AcceleratorType, GPUsPerReplica []int32 // [V]
+	ScaleToZeroEnabled, RequestError  []bool  // [M]
+	RequestCount                      []float64 // [M]
+	TypeLimit                         []int32 // [T] TypeInventory limits after Refresh
+	EnableLimiter                     bool
+}
+
+// SetDecisionInputs copies one cycle's decision columns into the page-locked arena (before Commit).
+func (g *Ingest) SetDecisionInputs(in *IngestDecisionInputs) {
+	v, m, t := g.nv, g.nm, int(g.dcols.n_types)
+	copy(unsafe.Slice((*int32)(unsafe.Pointer(g.dcols.var_accelerator_type)), v), in.AcceleratorType)
+	copy(unsafe.Slice((*int32)(unsafe.Pointer(g.dcols.var_gpus_per_replica)), v), in.GPUsPerReplica)
+	s2z := unsafe.Slice((*uint8)(unsafe.Pointer(g.dcols.mod_scale_to_zero_enabled)), m)
+	rerr := unsafe.Slice((*uint8)(unsafe.Pointer(g.dcols.mod_request_error)), m)
+	for i := 0; i < m; i++ {
+		s2z[i], rerr[i] = 0, 0
+		if in.ScaleToZeroEnabled[i] {
+			s2z[i] = 1
+		}
+		if in.RequestError[i] {
+			rerr[i] = 1
+		}
+	}
+	copy(unsafe.Slice((*float64)(unsafe.Pointer(g.dcols.mod_request_count)), m), in.RequestCount)
+	if t > 0 {
+		copy(unsafe.Slice((*int32)(unsafe.Pointer(g.dcols.type_limit)), t), in.TypeLimit)
+	}
+	en := int32(0)
+	if in.EnableLimiter {
+		en = 1
+	}
+	*(*int32)(unsafe.Pointer(g.dcols.enable_limiter)) = en
+}
+
+// IngestDecision: the numeric fields of one interfaces.VariantDecision after the cycle; the caller attaches the names
+// (VariantName, ModelID, Namespace, AcceleratorName) from the registry and the Reason / DecisionSteps strings.
+type IngestDecision struct {
+	Variant                                  int // registry index
+	OriginalTarget, Target, GPUsAllocated    int
+	Action                                   int // 1 scale-up, -1 scale-down, 0 no-change (before the limiter)
+	WasLimited                               bool
+}
+
+// Decisions: the cycle's final decisions in registry order, valid after Commit until the next Commit.
+func (g *Ingest) Decisions() []IngestDecision {
+	v := g.nv
+	has := unsafe.Slice((*uint8)(unsafe.Pointer(g.dres.has_decision)), v)
+	orig := unsafe.Slice((*int32)(unsafe.Pointer(g.dres.original_target)), v)
+	tgt := unsafe.Slice((*int32)(unsafe.Pointer(g.dres.target)), v)
+	gpus := unsafe.Slice((*int32)(unsafe.Pointer(g.dres.gpus_allocated)), v)
+	lim := unsafe.Slice((*uint8)(unsafe.Pointer(g.dres.was_limited)), v)
+	act := unsafe.Slice((*int8)(unsafe.Pointer(g.dres.action)), v)
+	var out []IngestDecision
+	for i := 0; i < v; i++ {
+		if has[i] == 0 {
+			continue
+		}
+		out = append(out, IngestDecision{Variant: i, OriginalTarget: int(orig[i]), Target: int(tgt[i]),
+			GPUsAllocated: int(gpus[i]), Action: int(act[i]), WasLimited: lim[i] != 0})
+	}
+	return out
 }

@@ -10,6 +10,7 @@ Records are plain dicts carrying the reference's Go field names (`PodName`, `KvC
 `TargetReplicas`, `GPUsPerReplica`, `SpareCapacity`, `GPUsAllocated`, `WasLimited`, `LimitedBy`, `DecisionSteps`), so a
 case from analyzer_test.go / default_limiter_test.go transcribes field by field.  Python twin of
 `go/wvab200/wvab200.go`; grouping, ordering and strings only — the arithmetic is `wva_saturation_v1` / `wva_limit`.
+`ingest_decisions` is the string side of the ingest graph's decision mode (the whole optimizeV1 tail on the device).
 """
 from __future__ import annotations
 
@@ -184,6 +185,43 @@ class Limiter:
             d.setdefault("DecisionSteps", []).append({"Name": self._name, "Action": d.get("Action", ""),
                                                       "TargetReplicas": d["TargetReplicas"], "Reason": self._reason(d),
                                                       "WasConstrained": d["WasLimited"]})
+
+
+ACTION_NAMES = {1: "scale-up", -1: "scale-down", 0: "no-change"}     # interfaces.SaturationAction (saturation_analyzer.go:222-224)
+
+
+def ingest_decisions(ing, models, variant_names, accelerator_names, limiter_name="gpu-limiter"):
+    """The tail of optimizeV1 (engines/saturation/engine.go:322-392) as VariantDecision dicts, from a decision-mode
+    `Ingest` after `commit()`: the device ran EnforcePolicy, convertSaturationTargetsToDecisions (:589-661) and the GPU
+    limiter; this attaches the strings.  models: [(ModelID, Namespace)] per registry model; variant_names /
+    accelerator_names: per registry variant (the AcceleratorName of the variant's analysis — read only for variants
+    that reported, the others carry "" as `va == nil` does, :647-655).  `limiter_name` = the DefaultLimiter's name
+    (engine.go:113).  Decisions come in registry order (the reference appends them per model in map order)."""
+    r, d, c, cols = ing.res, ing.dres, ing.dcols, ing.cols
+    mvo = np.asarray(ing.model_variant_off)
+    limited_on = bool(c["enable_limiter"][0])
+    out = []
+    for v in np.flatnonzero(d["has_decision"]):
+        v = int(v)
+        m = int(np.searchsorted(mvo, v, side="right")) - 1
+        va = int(r["var_replica_count"][v]) > 0
+        g = int(c["var_gpus_per_replica"][v])
+        action = ACTION_NAMES[int(d["action"][v])]
+        dec = {"VariantName": variant_names[v], "ModelID": models[m][0], "Namespace": models[m][1],
+               "CurrentReplicas": int(cols["var_current"][v]), "TargetReplicas": int(d["target"][v]),
+               "OriginalTargetReplicas": int(d["original_target"][v]), "DesiredReplicas": int(cols["var_desired"][v]),
+               "Action": action, "Reason": "saturation-only mode: " + action, "GPUsPerReplica": g if g > 0 else 1,
+               "AcceleratorName": accelerator_names[v] if va else "", "Cost": float(cols["var_cost"][v]) if va else 0.0,
+               "SpareCapacity": float(r["var_avg_spare_kv"][v]) if va else 0.0,
+               "GPUsAllocated": int(d["gpus_allocated"][v]), "WasLimited": bool(d["was_limited"][v]), "LimitedBy": "",
+               "DecisionSteps": []}
+        if limited_on:                                # DefaultLimiter.updateDecisionMetadata (default_limiter.go:85-97)
+            if dec["WasLimited"]:
+                dec["LimitedBy"] = limiter_name
+            dec["DecisionSteps"].append({"Name": limiter_name, "Action": action, "TargetReplicas": dec["TargetReplicas"],
+                                         "Reason": Limiter._reason(dec), "WasConstrained": dec["WasLimited"]})
+        out.append(dec)
+    return out
 
 
 # ======================================================================================================================
