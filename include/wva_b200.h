@@ -73,7 +73,8 @@ typedef struct wva_ctx wva_ctx;
 typedef struct wva_system {
   /* accelerators: AcceleratorSpec (types.go:29-37) */
   int32_t n_acc;
-  int32_t n_types;
+  int32_t n_types;                  /* T <= 64: wva_load_system returns WVA_ERR_LIMIT
+                                       for more (the allocators keep 64-bit type masks) */
   const float* acc_cost;            /* [A] Cost, cents/hr                         */
   const int32_t* acc_multiplicity;  /* [A] Multiplicity                           */
   const int32_t* acc_type;          /* [A] index of Type in [0,T)                 */

@@ -234,7 +234,7 @@ int32_t wva_last_timing(const wva_ctx* ctx, wva_timing* out) {
 int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   if (!ctx || !s) return WVA_ERR_ARG;
   if (s->n_acc < 0 || s->n_types < 0 || s->n_models < 0 || s->n_servers < 0) return WVA_ERR_ARG;
-  if (s->n_types > WVA_MAX_TYPES) return WVA_ERR_LIMIT;
+  if (s->n_types > WVA_MAX_TYPES) { ctx->last_error = "wva_load_system: more than 64 capacity types"; return WVA_ERR_LIMIT; }
   CK(cudaSetDevice(ctx->device));
   const size_t A = s->n_acc, T = s->n_types, M = s->n_models, S = s->n_servers, MA = M * A;
   struct Item { const void* src; size_t bytes; size_t off; };

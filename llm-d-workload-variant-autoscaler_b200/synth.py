@@ -98,7 +98,8 @@ def limit_capacity(sysd: dict, unconstrained_type_count, fraction: float = 0.6):
 def shard_system(sysd: dict, rank: int, world: int):
     """Model-sharded partition (SURVEY §8e): servers s with s % world == rank, tables replicated.
 
-    Models are 1:1 with servers in the synthetic systems, so the perf rows are sharded with them.
+    The shard keeps the perf rows of the models its servers run, once per model, and renumbers them.  A server with an
+    unknown model (srv_model < 0) keeps -1: it has no candidates, as in the whole system (Server.Calculate).
     """
     S, A = int(sysd["n_servers"]), int(sysd["n_acc"])
     idx = np.arange(rank, S, world)
@@ -106,12 +107,16 @@ def shard_system(sysd: dict, rank: int, world: int):
     for k, v in sysd.items():
         if k.startswith("srv_"):
             out[k] = np.asarray(v)[idx]
-    midx = np.asarray(sysd["srv_model"])[idx]
+    smod = np.asarray(sysd["srv_model"])[idx]
+    known = smod >= 0
+    models, local = np.unique(smod[known], return_inverse=True)
     for k in ("perf_alpha", "perf_beta", "perf_gamma", "perf_max_batch", "perf_at_tokens", "perf_acc_count",
               "perf_present"):
-        out[k] = np.asarray(sysd[k]).reshape(int(sysd["n_models"]), A)[midx]
-    out["srv_model"] = np.arange(len(idx), dtype=np.int32)
-    out["n_models"] = len(idx)
+        out[k] = np.ascontiguousarray(np.asarray(sysd[k]).reshape(int(sysd["n_models"]), A)[models])
+    sm = np.full(len(idx), -1, dtype=np.int32)
+    sm[known] = local
+    out["srv_model"] = sm
+    out["n_models"] = len(models)
     out["n_servers"] = len(idx)
     return out, idx
 
