@@ -288,7 +288,7 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
   extern __shared__ __align__(16) float grid_tiles[];
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned tile = (unsigned)__cvta_generic_to_shared(grid_tiles + (size_t)warp * (2 * 32 * 33));
+  const unsigned tile = (unsigned)__cvta_generic_to_shared(grid_tiles + (size_t)warp * TileTable::kWarpFloats);
   unsigned long long my_solves = 0, my_states = 0, my_slots = 0, my_rounds = 0;
   while (true) {
     unsigned long long i0 = 0;

@@ -51,38 +51,50 @@ struct LaneTable {   // one float32 column per lane ([n][thread], bank = lane); 
   __device__ __forceinline__ void prepare(int) const {}
 };
 // Rows in global memory, one per pool slot, and any 32 of them solved together (sizer_pool_kernel.cuh): the warp keeps
-// two shared tiles of 32 head states x 32 lanes ([state][lane], padded: conflict-free).  Tile k+1 is fetched with
-// cp.async (row by row: each row a coalesced 128-byte access, no registers, no scoreboard) while the lanes work on
-// tile k, so the only exposed latency is the first tile of a pass.  The tile is held as a shared-space address and
-// read with ld.shared (a generic pointer would be read with generic loads), and the table is passed by value, so that
-// a __noinline__ solver keeps its fields in registers.
+// two shared tiles of 32 head states x 32 lanes.  Tile k+1 is fetched with cp.async (no registers, no scoreboard) while
+// the lanes work on tile k, so the only exposed latency is the first tile of a pass.  A tile is lane-major: lane l's 32
+// states are 8 chunks of 4 states (16 bytes) at l * 128 bytes, chunk c stored in place c ^ (l & 7), so that the
+// 16-byte reads of 8 consecutive lanes hit 8 different bank quads (conflict-free) and a chunk of 16 states is 4 loads.
+// The fetch moves 4 rows per cp.async instruction (8 lanes x 16 bytes per row: coalesced 128-byte accesses), 8
+// instructions and 8 shuffles of the row index per tile.  The tile is held as a shared-space address and read with
+// ld.shared (a generic pointer would be read with generic loads), and the table is passed by value, so that a
+// __noinline__ solver keeps its fields in registers.  Only (E1) rows are read through it (the pool queues and the
+// deferred grid pass take no other pair), so the loads convert on the integer pipe (f32pos_to_d, rcp_f32den_e1).
 struct TileTable {
   static constexpr int kChunk = WVA_TILE_CHUNK;   // states per unrolled chunk of the solver (code size vs loop overhead)
-  static_assert(32 % kChunk == 0, "a chunk lies inside one tile");
-  const float* rows;      // base of the CTA's rows
+  static constexpr int kWarpFloats = 2 * 32 * 32; // shared floats per warp (two tiles)
+  static_assert(32 % kChunk == 0 && kChunk % 4 == 0, "a chunk lies inside one tile and is whole 16-byte groups");
+  const float* rows;      // base of the CTA's rows (16-byte aligned)
   int row_stride;         // floats per row (a multiple of 32, >= N)
   int slot;               // this lane's row (any valid row for an idle lane)
-  unsigned tile;          // shared-space address of the warp's two [32][33] tiles
+  unsigned tile;          // shared-space address of the warp's two tiles (kWarpFloats, 16-byte aligned)
   int n_head;             // head entries (N - 1): tiles beyond are never fetched
+  // shared address of the 16 bytes of lane l's row holding states n .. n+3 (n a multiple of 4)
+  __device__ __forceinline__ unsigned group_addr(unsigned l, int n) const {
+    return tile + (((unsigned)n >> 5) & 1u) * 4096u + l * 128u + (((((unsigned)n >> 2) & 7u) ^ (l & 7u)) << 4);
+  }
   __device__ __forceinline__ void fetch(int n0) const {
-    const int lane = threadIdx.x & 31;
-    const unsigned dst0 = tile + 4u * (((n0 >> 5) & 1) * (32 * 33) + lane * 33);
-#pragma unroll 8
-    for (int r = 0; r < 32; r++) {
-      const int sr = __shfl_sync(0xffffffffu, slot, r);
-      const float* src = rows + (size_t)sr * row_stride + n0 + lane;
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst0 + 4u * r), "l"(src) : "memory");
+    const unsigned lane = threadIdx.x & 31, c = lane & 7;
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+      const unsigned l = 4 * k + (lane >> 3);      // the row (lane) this lane copies 16 bytes of
+      const int sr = __shfl_sync(0xffffffffu, slot, l);
+      const float* src = rows + (size_t)sr * row_stride + n0 + 4 * c;
+      asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(group_addr(l, n0 + 4 * c)), "l"(src) : "memory");
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   }
   // shared address of this lane's entry of state n
-  __device__ __forceinline__ unsigned addr(int n) const {
-    return tile + 4u * (((n >> 5) & 1) * (32 * 33) + (n & 31) * 33 + (threadIdx.x & 31));
-  }
+  __device__ __forceinline__ unsigned addr(int n) const { return group_addr(threadIdx.x & 31, n & ~3) + 4u * (n & 3); }
   // volatile: kept after the cp.async wait and __syncwarp of prepare()
   static __device__ __forceinline__ float lds(unsigned a) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
+    return v;
+  }
+  static __device__ __forceinline__ float4 lds4(unsigned a) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
     return v;
   }
   __device__ __forceinline__ void prepare(int n) const {
@@ -102,15 +114,19 @@ struct TileTable {
     __syncwarp();
   }
   __device__ __forceinline__ void load(int n, double& mu, double& r) const {
-    float m32 = lds(addr(n)); mu = (double)m32; r = rcp_f32den(m32, mu);
+    float m32 = lds(addr(n)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
   }
-  // state n + j sits j rows of 33 floats below state n: one address per chunk, immediate offsets after it
   template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
-    const unsigned a = addr(n);
+    const unsigned l = threadIdx.x & 31;
 #pragma unroll
-    for (int j = 0; j < CH; j++) { float m32 = lds(a + 4u * 33u * j); mu[j] = (double)m32; r[j] = rcp_f32den(m32, mu[j]); }
+    for (int g = 0; g < CH / 4; g++) {
+      const float4 v = lds4(group_addr(l, n + 4 * g));
+      const float m32[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 4; e++) { mu[4 * g + e] = f32pos_to_d(m32[e]); r[4 * g + e] = rcp_f32den_e1(m32[e], mu[4 * g + e]); }
+    }
   }
-  __device__ __forceinline__ double mu_at(int n) const { return (double)lds(addr(n)); }
+  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(lds(addr(n))); }
 };
 
 // high word of v * 2^-54 for a normal v >= 2^-900: the exponent field moves, nothing rounds

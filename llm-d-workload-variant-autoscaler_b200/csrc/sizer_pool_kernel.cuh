@@ -43,8 +43,9 @@ struct PoolSmem {
   unsigned short free_list[POOL_PMAX];
   int head[POOL_NCLS], tail[POOL_NCLS];
   int n_free, in_pool, exhausted, lock;
-  float tiles[POOL_THREADS / 32][2 * 32 * 33];
+  float tiles[POOL_THREADS / 32][TileTable::kWarpFloats];
 };
+static_assert(offsetof(PoolSmem, tiles) % 16 == 0, "TileTable's tiles take 16-byte cp.async copies and loads");
 
 __device__ __forceinline__ void pool_lock(int* lock) {
   if ((threadIdx.x & 31) == 0) {

@@ -111,6 +111,22 @@ WVA_HD double rcp_refine(float s, double mu) {
 // 1/mu is not a float32 normal number and the seed flushes: a subnormal mu reads as 0 (seed inf, r = NaN), mu > 2^126
 // has a subnormal 1/mu (seed 0, r = 0), and mu = inf gives r = NaN.
 WVA_HD double rcp_f32den(float m32, double mu) { return rcp_refine(f_rcp_approx(m32), mu); }
+// (double)v for a positive normal float32 v, as every (E1) divisor and its rcp seed are (e1_divisor: [2^-126, 2^126]).  The
+// exponent is rebiased and the significand shifted on the integer pipe — the same bits as the conversion, which on H100
+// issues to the FP64 pipe at a quarter of the DFMA rate (CUDA C++ Programming Guide, arithmetic instruction throughput).
+WVA_HD double f32pos_to_d(float v) {
+#if defined(__CUDA_ARCH__)
+  const unsigned b = __float_as_uint(v);
+  return __hiloint2double((int)((b >> 3) + 0x38000000u), (int)(b << 29));
+#else
+  return (double)v;
+#endif
+}
+// rcp_f32den of an (E1) divisor with both conversions on the integer pipe: the same bits as rcp_f32den(m32, (double)m32)
+WVA_HD double rcp_f32den_e1(float m32, double mu) {
+  const double r0 = f32pos_to_d(f_rcp_approx(m32));
+  return d_fma(r0, d_fma(-mu, r0, 1.0), r0);
+}
 // mu in [2^-126, 2^126]: the divisors (E1) holds for
 WVA_HD bool e1_divisor(float m32) {
 #if defined(__CUDA_ARCH__)
