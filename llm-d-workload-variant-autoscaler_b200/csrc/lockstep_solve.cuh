@@ -630,12 +630,5 @@ __device__ __noinline__ int lockstep_solve_fast_only(const PairModel& m, const T
   return cert || !active ? states : -1 - states;
 }
 
-// evaluation values of a finished solve (EvalTTFT / EvalITL, queueanalyzer.go:283-308)
-__device__ __forceinline__ void eval_values(const PairModel& m, const SolveStats& st, float* ttft, float* itl, float* pf) {
-  *pf = prefill_time(m, st.avgNumInServers);
-  *itl = f_div(f_sub(st.avgServTime, *pf), m.out_tok);
-  *ttft = f_add(f_add(st.avgWaitTime, *pf), *itl);
-}
-
 #endif  // __CUDACC__
 }  // namespace wva

@@ -24,6 +24,16 @@ struct SizerCounters {
   unsigned long long certify_fallbacks; // pool sizer: fast solves (E12) not certified, redone by the exact solver
 };
 
+// A pair whose chain overflowed float64 (`states` = states of the failed solve or round): counted, listed for
+// overflow_slow_kernel (which redoes it with the reference's rescale) and written as nil until then.
+__device__ __forceinline__ void retire_overflow(SizerLane& z, const SysView& s, const CandView& out, SizerCounters* ctr,
+                                                int* overflow_list, int states) {
+  const unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
+  if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
+  z.states += states;
+  lane_fail(z, s, out);
+}
+
 // Largest max-batch-size N any pair that needs sizing will use (allocation.go:79-88):
 // decides the table geometry of the sizer launch.
 __global__ void __launch_bounds__(256) max_batch_kernel(SysView s, unsigned long long n_pairs, int* out) {
@@ -108,10 +118,7 @@ sizer_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, floa
       if (live) {
         if (chain_step(z.c, z.m, st)) {
           if (z.c.phase == CH_OVERFLOW) {
-            unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
-            if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
-            z.states += z.c.states;
-            lane_fail(z, s, out);
+            retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
             live = false;
           } else {
             live = sizer_on_solve(z, s, out, st);

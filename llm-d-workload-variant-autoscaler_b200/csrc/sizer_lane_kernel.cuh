@@ -114,9 +114,9 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
     int sv = 0;
     if (uniform && !live) { z.m.N = nref; z.m.K = nref + nref * WVA_QUEUE_TO_BATCH; }   // idle lanes only keep the loops uniform
     LaneTable lt; lt.t = tab; lt.stride = stride;
+    SolveStats st2[2];
     if (DUAL) {
       // TTFT and ITL searches advance together: two chains per lane share every table load
-      SolveStats st2[2];
       float xs[2] = {z.x2[0], z.x2[1]};
       bool act[2] = {live && z.act2[0], live && z.act2[1]};
       if (uniform) {
@@ -131,19 +131,6 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
           sv += z.c.states;
         }
       }
-      if (live) {
-        if (bad) {
-          unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
-          if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
-          z.states += sv;
-          lane_fail(z, s, out);
-          live = false;
-        } else {
-          live = SPLIT ? spec2_on_solve(z, s, out, st2, sv) : dual_on_solve(z, s, out, st2, sv);
-          if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<true>(z, s, out, sw); }
-        }
-        if (!live) { my_solves += z.solves; my_states += z.states; }
-      }
     } else {
       if (uniform) {
         lockstep_solve(z.m, lt, z.cur_x, live, st, sv, bad);
@@ -152,19 +139,16 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
         while (!chain_step(z.c, z.m, st)) {}
         bad = z.c.phase == CH_OVERFLOW;
       }
-      if (live) {
-        if (bad) {
-          unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
-          if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
-          z.states += z.c.states;
-          lane_fail(z, s, out);
-          live = false;
-        } else {
-          live = sizer_on_solve(z, s, out, st);
-          if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<false>(z, s, out, sw); }
-        }
-        if (!live) { my_solves += z.solves; my_states += z.states; }
+    }
+    if (live) {
+      if (bad) {
+        retire_overflow(z, s, out, ctr, overflow_list, DUAL ? sv : z.c.states);
+        live = false;
+      } else {
+        live = DUAL ? (SPLIT ? spec2_on_solve(z, s, out, st2, sv) : dual_on_solve(z, s, out, st2, sv)) : sizer_on_solve(z, s, out, st);
+        if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<DUAL>(z, s, out, sw); }
       }
+      if (!live) { my_solves += z.solves; my_states += z.states; }
     }
     {
       int mxs = sv;

@@ -144,10 +144,7 @@ __device__ __noinline__ bool pool_pair_on_chain(PoolEntry& ze, const SysView& s,
   while (live) {
     while (!chain_step(z.c, z.m, st)) {}
     if (z.c.phase == CH_OVERFLOW) {
-      const unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
-      if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
-      z.states += z.c.states;
-      lane_fail(z, s, out);
+      retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
       live = false;
     } else {
       live = sizer_on_solve(z, s, out, st);
@@ -322,11 +319,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       if (need_table) {
         PairModel& m = z.m;
         m.tab = rows + (size_t)new_slot * row_stride; m.stride = 1;
-        const float lmin = f_mul(r0, WVA_EPSILON), lmax = f_mul(rl, f_sub(1.0f, WVA_EPSILON));     // queueanalyzer.go:107-108
-        const float rmin = f_mul(lmin, 1000.0f);
-        m.rate_max = f_mul(lmax, 1000.0f);
-        m.lambda_min = f_div(rmin, 1000.0f);                                                         // :189-190
-        m.lambda_max = f_div(m.rate_max, 1000.0f);
+        model_set_range(m, r0, rl);
         m.mono = mono;
         // every entry an (E1) divisor?  The row is non-decreasing from mono on, so its ends bound it there; read through
         // L2, where the lanes wrote it (L1 may still hold the slot's previous row)
@@ -407,10 +400,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       }
       bool cont;
       if (bad) {
-        const unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
-        if (overflow_list) overflow_list[k] = z.srv * s.n_acc + z.acc;
-        z.states += z.c.states;
-        lane_fail(z, s, out);
+        retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
         cont = false;
       } else {
         cont = sizer_on_solve(z, s, out, st);

@@ -79,22 +79,15 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
     __syncwarp();
     model_finish(m, tabf, 1);
     const size_t idx = (size_t)srv * s.n_acc + acc;
-    Alloc fail; fail.state = ALLOC_NONE; fail.num_replicas = 0; fail.batch_size = 0;
-    fail.cost = fail.value = fail.itl = fail.ttft = fail.rho = fail.max_arrv = 0.0f;
     int solves = 0;
     bool failed = false, ovf_any = false;
-
-    Search sT, sI;
-    sT.target = z.sT.target; sI.target = z.sI.target;
-    sT.enabled = sT.target > 0.0f; sI.enabled = sI.target > 0.0f;
-    sT.active = sT.enabled; sI.active = sI.enabled;
-    sT.result = m.lambda_max; sI.result = m.lambda_max;
-    sT.iter = sI.iter = 0;
+    Search& sT = z.sT;
+    Search& sI = z.sI;
     SolveStats st;
     bool ovf;
     float y_t, y_i, pf;
 
-    if (sT.enabled || sI.enabled) {
+    if (searches_begin(z)) {
       if (m.lambda_min > m.lambda_max) failed = true;   // BinarySearch: invalid range (utils.go:29-31)
       else {
         // ---- round 0: both end points (lanes 0,1) + the first 4 levels of the tree shared by both
@@ -114,16 +107,8 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
             Search& q = k ? sI : sT;
             if (!q.active) continue;
             const float my_y = k ? y_i : y_t;
-            const float y_lo = __shfl_sync(full, my_y, 0), y_hi = __shfl_sync(full, my_y, 1);
-            // the reference evaluates xMin first and returns before touching xMax when it matches
-            if (within_tolerance(y_lo, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_min; q.active = false; continue; }
-            if (within_tolerance(y_hi, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_max; q.active = false; continue; }
-            q.increasing = y_lo < y_hi;
-            if ((q.increasing && q.target < y_lo) || (!q.increasing && q.target > y_lo)) { failed = true; q.active = false; continue; }
-            if ((q.increasing && q.target > y_hi) || (!q.increasing && q.target < y_hi)) { q.result = m.lambda_max; q.active = false; continue; }
-            q.lo = m.lambda_min; q.hi = m.lambda_max; q.iter = 0;
-            q.x = f_mul(0.5f, f_add(q.lo, q.hi));
-            spec_walk(q, D0, [&](int node) { return __shfl_sync(full, my_y, node + 1); });
+            if (!search_bracket(q, m, __shfl_sync(full, my_y, 0), __shfl_sync(full, my_y, 1))) failed = true;
+            else if (q.active) spec_walk(q, D0, [&](int node) { return __shfl_sync(full, my_y, node + 1); });
           }
         }
         // ---- further rounds: 15-node trees, TTFT on lanes 0..14, ITL on lanes 16..30 (31-node tree on
@@ -153,42 +138,22 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       }
     }
     // ---- Size() tail + CreateAllocation (queueanalyzer.go:232-247, allocation.go:123-153) --------------
-    Alloc a = fail;
+    Alloc a = alloc_none();
+    float x;
     if (!failed && !ovf_any) {
-      float l_tps = m.lambda_max;
-      if (z.slo_tps > 0.0f) l_tps = f_mul(m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));
-      float lambda = fminf(fminf(sT.result, sI.result), l_tps);
-      float request_rate = f_mul(lambda, 1000.0f);
-      if (!analyze_admits(m, request_rate)) failed = true;
+      if (!size_lambda(z, x)) failed = true;
       else {
-        warp_solve(m, tab, f_div(request_rate, 1000.0f), lane == 0, st, sv_states, ovf); my_states += sv_states;
+        warp_solve(m, tab, x, lane == 0, st, sv_states, ovf); my_states += sv_states;
         solves++;
         if (__shfl_sync(full, (int)ovf, 0)) ovf_any = true;
+        else if (!alloc_replicas(z, __shfl_sync(full, st.throughput, 0), x)) failed = true;
         else {
-          float rate_star = __shfl_sync(full, f_mul(st.throughput, 1000.0f), 0);
-          long long nr = go_int_ceil(d_div((double)z.total_rate, (double)rate_star));
-          if (nr < (long long)z.min_replicas) nr = z.min_replicas;
-          long long tot = (long long)((unsigned long long)z.n_inst * (unsigned long long)nr);
-          float cost = f_mul(z.acc_cost, (float)tot);
-          float rate = f_div(z.total_rate, (float)nr);
-          if (!analyze_admits(m, rate)) failed = true;
-          else {
-            warp_solve(m, tab, f_div(rate, 1000.0f), lane == 0, st, sv_states, ovf); my_states += sv_states;
-            solves++;
-            if (__shfl_sync(full, (int)ovf, 0)) ovf_any = true;
-            else if (lane == 0) {
-              eval_values(m, st, &y_t, &y_i, &pf);
-              a.state = ALLOC_ACC;
-              a.num_replicas = nr;
-              a.batch_size = m.N;
-              a.cost = cost;
-              a.itl = y_i;
-              a.ttft = f_add(st.avgWaitTime, pf);
-              float rho = f_div(st.avgNumInServers, (float)m.N);
-              a.rho = fminf(fmaxf(rho, 0.0f), 1.0f);
-              a.max_arrv = f_div(rate_star, 1000.0f);
-              a.value = transition_penalty(s.srv_cur_acc[srv], s.srv_cur_replicas[srv], s.srv_cur_cost[srv], a, acc);
-            }
+          warp_solve(m, tab, x, lane == 0, st, sv_states, ovf); my_states += sv_states;
+          solves++;
+          if (__shfl_sync(full, (int)ovf, 0)) ovf_any = true;
+          else if (lane == 0) {
+            eval_values(m, st, &y_t, &y_i, &pf);
+            a = alloc_final(z, s, st, y_i, pf);
           }
         }
       }
@@ -197,10 +162,8 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       if (ovf_any) {
         unsigned long long k = atomicAdd(&ctr->overflow_pairs, 1ull);
         if (overflow_list) overflow_list[k] = (int)idx;
-        store_candidate(out, idx, fail, solves);
-      } else {
-        store_candidate(out, idx, a, solves);   // a == fail when the pair is infeasible
       }
+      store_candidate(out, idx, a, solves);   // nil when the pair is infeasible or overflowed
       my_solves += (unsigned long long)solves;
     }
     __syncwarp();

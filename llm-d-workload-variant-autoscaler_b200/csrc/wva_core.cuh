@@ -212,17 +212,20 @@ WVA_HD float serv_rate(const PairModel& m, int n) {
 WVA_HD void model_fill_table(const PairModel& m, float* tab, int stride, int first, int step) {
   for (int n = first; n < m.N; n += step) tab[(size_t)n * stride] = serv_rate(m, n + 1);
 }
-// finish the model once the table is complete
-WVA_HD void model_finish(PairModel& m, const float* tab, int stride) {
-  m.tab = tab; m.stride = stride;
-  float r0 = tab[0];
-  float rl = tab[(size_t)(m.N - 1) * stride];
+// RateRange of BuildModel from the first and last service rate r0, rl, and Size()'s lambda range
+WVA_HD void model_set_range(PairModel& m, float r0, float rl) {
   float lmin = f_mul(r0, WVA_EPSILON);                       // queueanalyzer.go:107
   float lmax = f_mul(rl, f_sub(1.0f, WVA_EPSILON));          // queueanalyzer.go:108
   float rmin = f_mul(lmin, 1000.0f);                         // :109 RateRange{Min,Max}
   m.rate_max = f_mul(lmax, 1000.0f);
   m.lambda_min = f_div(rmin, 1000.0f);                       // Size(): queueanalyzer.go:189-190
   m.lambda_max = f_div(m.rate_max, 1000.0f);
+}
+// finish the model once the table is complete
+WVA_HD void model_finish(PairModel& m, const float* tab, int stride) {
+  m.tab = tab; m.stride = stride;
+  float rl = tab[(size_t)(m.N - 1) * stride];
+  model_set_range(m, tab[0], rl);
   int mono = 0;
   float nxt = rl;
   for (int n = m.N - 2; n >= 0; n--) {
@@ -610,6 +613,13 @@ struct Alloc {  // core.Allocation (pkg/core/allocation.go:13-24)
   float cost, value, itl, ttft, rho, max_arrv;
 };
 
+// the nil allocation: no candidate on this accelerator
+WVA_HD Alloc alloc_none() {
+  Alloc a; a.state = ALLOC_NONE; a.num_replicas = 0; a.batch_size = 0;
+  a.cost = a.value = a.itl = a.ttft = a.rho = a.max_arrv = 0.0f;
+  return a;
+}
+
 WVA_HD int sat_i32(long long v) {
   return v > 2147483647LL ? 2147483647 : (v < -2147483647LL - 1 ? (-2147483647 - 1) : (int)v);
 }
@@ -698,8 +708,7 @@ WVA_HD int sizer_setup(SizerLane& z, const SysView& s, const CandView& out, int 
   z.srv = srv; z.acc = acc; z.solves = 0; z.states = 0;
   z.split = -1; z.merged = false; z.failed = false;
   size_t idx = (size_t)srv * s.n_acc + acc;
-  Alloc a; a.state = ALLOC_NONE; a.num_replicas = 0; a.batch_size = 0;
-  a.cost = a.value = a.itl = a.ttft = a.rho = a.max_arrv = 0.0f;
+  Alloc a = alloc_none();
   int cur_acc = s.srv_cur_acc[srv];
   // Server.GetCandidateAccelerators (server.go:70-82)
   bool restricted = s.srv_keep_acc[srv] && cur_acc != -1;
@@ -771,15 +780,8 @@ WVA_HD void lane_start_solve(SizerLane& z, float lambda) {
 }
 
 WVA_HD void lane_fail(SizerLane& z, const SysView& s, const CandView& out) {
-  Alloc a; a.state = ALLOC_NONE; a.num_replicas = 0; a.batch_size = 0;
-  a.cost = a.value = a.itl = a.ttft = a.rho = a.max_arrv = 0.0f;
-  store_candidate(out, (size_t)z.srv * s.n_acc + z.acc, a, z.solves);
+  store_candidate(out, (size_t)z.srv * s.n_acc + z.acc, alloc_none(), z.solves);
 }
-
-// After the table is built: start Size() (queueanalyzer.go:181-258).  Returns false
-// if the pair finished without needing a solve.
-WVA_HD bool sizer_begin(SizerLane& z, const SysView& s, const CandView& out);
-WVA_HD bool sizer_after_search(SizerLane& z, const SysView& s, const CandView& out);
 
 // a failure during the search phase: in split mode it is published for the partner item instead of written
 WVA_HD bool search_fail(SizerLane& z, const SysView& s, const CandView& out) {
@@ -788,35 +790,51 @@ WVA_HD bool search_fail(SizerLane& z, const SysView& s, const CandView& out) {
   return false;
 }
 
-WVA_HD bool sizer_begin(SizerLane& z, const SysView& s, const CandView& out) {
+// Analyze() pre-checks (queueanalyzer.go:128-136)
+WVA_HD bool analyze_admits(const PairModel& m, float rate) { return rate > 0.0f && !(rate > m.rate_max); }
+
+// ---- the steps of Size() and CreateAllocation, shared by every sizer driver -------------------------------------
+
+// EvalTTFT / EvalITL of a finished solve, and the prefill time Analyze adds to the waiting time
+// (queueanalyzer.go:143-149,283-308)
+WVA_HD void eval_values(const PairModel& m, const SolveStats& st, float* ttft, float* itl, float* pf) {
+  *pf = prefill_time(m, st.avgNumInServers);
+  *itl = f_div(f_sub(st.avgServTime, *pf), m.out_tok);
+  *ttft = f_add(f_add(st.avgWaitTime, *pf), *itl);
+}
+
+// Size()'s two BinarySearch calls (queueanalyzer.go:197-230): a search runs when its target is positive, and a split
+// item runs only its own.  Returns false when neither runs.
+WVA_HD bool searches_begin(SizerLane& z) {
   z.sT.enabled = z.sT.target > 0.0f && z.split != 1;
   z.sI.enabled = z.sI.target > 0.0f && z.split != 0;
   z.sT.active = z.sT.enabled; z.sI.active = z.sI.enabled;
   z.sT.result = z.m.lambda_max; z.sI.result = z.m.lambda_max;
   z.sT.iter = z.sI.iter = 0;
-  if (z.sT.enabled || z.sI.enabled) {
-    // BinarySearch: xMin > xMax -> error (utils.go:29-31)
-    if (z.m.lambda_min > z.m.lambda_max) return search_fail(z, s, out);
-    z.stage = SZ_LO;
-    lane_start_solve(z, z.m.lambda_min);
-    return true;
-  }
-  return sizer_after_search(z, s, out);
+  return z.sT.enabled || z.sI.enabled;
 }
 
-// Analyze() pre-checks (queueanalyzer.go:128-136)
-WVA_HD bool analyze_admits(const PairModel& m, float rate) { return rate > 0.0f && !(rate > m.rate_max); }
-
-WVA_HD bool sizer_after_search(SizerLane& z, const SysView& s, const CandView& out) {
-  if (z.split >= 0 && !z.merged) { z.stage = SZ_PUBLISH; return true; }   // publish; the second finisher goes on
-  float l_tps = z.m.lambda_max;
-  if (z.slo_tps > 0.0f) l_tps = f_mul(z.m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));  // :232-235
-  float lambda = fminf(fminf(z.sT.result, z.sI.result), l_tps);                             // :238
-  float request_rate = f_mul(lambda, 1000.0f);                                               // :239
-  if (!analyze_admits(z.m, request_rate)) { lane_fail(z, s, out); return false; }
-  z.stage = SZ_FINAL1;
-  lane_start_solve(z, f_div(request_rate, 1000.0f));                                         // :139
+// BinarySearch's end points (utils.go:33-57), xMin first: when f(xMin) is within tolerance the search ends at xMin and
+// the reference never evaluates xMax.
+WVA_HD void search_lo(Search& q, const PairModel& m, float y_lo) {
+  q.y_lo = y_lo;
+  if (within_tolerance(y_lo, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_min; q.active = false; }
+}
+// xMax, for a search search_lo left active: within tolerance or a target above the bounded region ends it at xMax; a
+// target below the region fails it (returns false); else the bisection starts on [xMin, xMax].
+WVA_HD bool search_hi(Search& q, const PairModel& m, float y_hi) {
+  if (within_tolerance(y_hi, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_max; q.active = false; return true; }
+  q.increasing = q.y_lo < y_hi;
+  if ((q.increasing && q.target < q.y_lo) || (!q.increasing && q.target > q.y_lo)) { q.active = false; return false; }  // ind = -1
+  if ((q.increasing && q.target > y_hi) || (!q.increasing && q.target < y_hi)) { q.result = m.lambda_max; q.active = false; return true; }  // ind = +1
+  q.lo = m.lambda_min; q.hi = m.lambda_max; q.iter = 0; q.y_hi = y_hi;
+  q.x = f_mul(0.5f, f_add(q.lo, q.hi));
   return true;
+}
+// both end points, evaluated in the same round; false when the search fails
+WVA_HD bool search_bracket(Search& q, const PairModel& m, float y_lo, float y_hi) {
+  search_lo(q, m, y_lo);
+  return !q.active || search_hi(q, m, y_hi);
 }
 
 // one search consumes the evaluation y = f(x) of the solve just finished
@@ -833,27 +851,126 @@ WVA_HD void search_consume(Search& q, float x, float y) {
   if (q.x == x) { q.result = x; q.active = false; }
 }
 
+// Size()'s tail (queueanalyzer.go:232-239) and Analyze's admission of its rate (:128-136): false when the rate is not
+// admitted, else x = the arrival rate of the first Analyze solve (:139)
+WVA_HD bool size_lambda(const SizerLane& z, float& x) {
+  float l_tps = z.m.lambda_max;
+  if (z.slo_tps > 0.0f) l_tps = f_mul(z.m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));  // :232-235
+  float lambda = fminf(fminf(z.sT.result, z.sI.result), l_tps);                             // :238
+  float request_rate = f_mul(lambda, 1000.0f);                                               // :239
+  if (!analyze_admits(z.m, request_rate)) return false;
+  x = f_div(request_rate, 1000.0f);
+  return true;
+}
+
+// CreateAllocation's replica count from the first Analyze solve (allocation.go:123-145): false when the rate per
+// replica is not admitted, else x = the arrival rate of the second Analyze solve
+WVA_HD bool alloc_replicas(SizerLane& z, float throughput, float& x) {
+  z.rate_star = f_mul(throughput, 1000.0f);                                           // allocation.go:123
+  long long nr = go_int_ceil(d_div((double)z.total_rate, (double)z.rate_star));       // :132
+  if (nr < (long long)z.min_replicas) nr = z.min_replicas;
+  z.num_replicas = nr;
+  long long tot = (long long)((unsigned long long)z.n_inst * (unsigned long long)nr);
+  z.cost = f_mul(z.acc_cost, (float)tot);
+  float rate = f_div(z.total_rate, (float)nr);
+  if (!analyze_admits(z.m, rate)) return false;
+  x = f_div(rate, 1000.0f);
+  return true;
+}
+
+// the allocation CreateAllocation returns, from the second Analyze solve st and its eval_values itl, pf
+// (allocation.go:146-153)
+WVA_HD Alloc alloc_final(const SizerLane& z, const SysView& s, const SolveStats& st, float itl, float pf) {
+  Alloc a;
+  a.state = ALLOC_ACC;
+  a.num_replicas = z.num_replicas;
+  a.batch_size = z.m.N;
+  a.cost = z.cost;
+  a.itl = itl;
+  a.ttft = f_add(st.avgWaitTime, pf);
+  float rho = f_div(st.avgNumInServers, (float)z.m.N);
+  a.rho = fminf(fmaxf(rho, 0.0f), 1.0f);
+  a.max_arrv = f_div(z.rate_star, 1000.0f);
+  a.value = transition_penalty(s.srv_cur_acc[z.srv], s.srv_cur_replicas[z.srv], s.srv_cur_cost[z.srv], a, z.acc);
+  return a;
+}
+
+// ---- sequential driver: one chain per lane, the solves of the two searches one after the other ----------------
+WVA_HD bool sizer_after_search(SizerLane& z, const SysView& s, const CandView& out) {
+  if (z.split >= 0 && !z.merged) { z.stage = SZ_PUBLISH; return true; }   // publish; the second finisher goes on
+  float x;
+  if (!size_lambda(z, x)) { lane_fail(z, s, out); return false; }
+  z.stage = SZ_FINAL1;
+  lane_start_solve(z, x);
+  return true;
+}
+
+// After the table is built: start Size() (queueanalyzer.go:181-258).  Returns false
+// if the pair finished without needing a solve.
+WVA_HD bool sizer_begin(SizerLane& z, const SysView& s, const CandView& out) {
+  if (!searches_begin(z)) return sizer_after_search(z, s, out);
+  // BinarySearch: xMin > xMax -> error (utils.go:29-31)
+  if (z.m.lambda_min > z.m.lambda_max) return search_fail(z, s, out);
+  z.stage = SZ_LO;
+  lane_start_solve(z, z.m.lambda_min);
+  return true;
+}
+
+// ---- two-chain drivers: the lane solves the arrival rates z.x2[c] where z.act2[c] in one round -----------------
+WVA_HD void dual_start1(SizerLane& z, float x) {   // one solve in the coming round
+  z.x2[0] = x; z.act2[0] = true; z.act2[1] = false;
+  z.solves++;
+}
+
+WVA_HD bool dual_after_search(SizerLane& z, const SysView& s, const CandView& out) {
+  float x;
+  if (!size_lambda(z, x)) { lane_fail(z, s, out); return false; }
+  z.stage = SZ_FINAL1;
+  dual_start1(z, x);
+  return true;
+}
+
+// a split item publishes its search's result first (split_publish); the item that finishes second goes on
+WVA_HD bool spec2_after_search(SizerLane& z, const SysView& s, const CandView& out) {
+  if (z.split >= 0 && !z.merged) { z.stage = SZ_PUBLISH; return true; }
+  return dual_after_search(z, s, out);
+}
+
+// round 0 evaluates both end points of every search the split item (or the whole pair) runs
+WVA_HD bool spec2_begin(SizerLane& z, const SysView& s, const CandView& out) {
+  if (!searches_begin(z)) return spec2_after_search(z, s, out);
+  if (z.m.lambda_min > z.m.lambda_max) return search_fail(z, s, out);   // utils.go:29-31
+  z.stage = SZ_LO;
+  z.x2[0] = z.m.lambda_min; z.x2[1] = z.m.lambda_max; z.act2[0] = z.act2[1] = true;
+  z.solves += 2;
+  return true;
+}
+// a whole pair starts as a split item does: the split steps do nothing for it
+WVA_HD bool dual_begin(SizerLane& z, const SysView& s, const CandView& out) { return spec2_begin(z, s, out); }
+
+// the two Analyze solves (stages SZ_FINAL1, SZ_FINAL2), on chain 0
+WVA_HD bool dual_final(SizerLane& z, const SysView& s, const CandView& out, const SolveStats& st) {
+  if (z.stage == SZ_FINAL1) {
+    float x;
+    if (!alloc_replicas(z, st.throughput, x)) { lane_fail(z, s, out); return false; }
+    z.stage = SZ_FINAL2;
+    dual_start1(z, x);
+    return true;
+  }
+  float ttft, itl, pf;
+  eval_values(z.m, st, &ttft, &itl, &pf);
+  const Alloc a = alloc_final(z, s, st, itl, pf);
+  store_candidate(out, (size_t)z.srv * s.n_acc + z.acc, a, z.solves);
+  return false;
+}
+
 // ---- dual-chain driver: TTFT and ITL searches advance in the SAME round (two chains per lane) -----
 // Used by the lock-step lane sizer.  Same decisions as sizer_on_solve (which runs the two searches one
 // after the other): both end points in round 0, then one bisection step of each search per round,
 // then the two Analyze solves.  ~30 rounds per pair instead of ~58 solves in sequence.
-enum { D2_ENDS = 0, D2_SEARCH = 1, D2_FINAL1 = 2, D2_FINAL2 = 3 };
-
-WVA_HD bool dual_after_search(SizerLane& z, const SysView& s, const CandView& out) {
-  float l_tps = z.m.lambda_max;
-  if (z.slo_tps > 0.0f) l_tps = f_mul(z.m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));   // queueanalyzer.go:232-235
-  float lambda = fminf(fminf(z.sT.result, z.sI.result), l_tps);                              // :238
-  float request_rate = f_mul(lambda, 1000.0f);                                                // :239
-  if (!analyze_admits(z.m, request_rate)) { lane_fail(z, s, out); return false; }
-  z.stage = D2_FINAL1;
-  z.x2[0] = f_div(request_rate, 1000.0f); z.act2[0] = true; z.act2[1] = false;
-  z.solves++;
-  return true;
-}
-
 WVA_HD bool dual_schedule(SizerLane& z, const SysView& s, const CandView& out) {
   if (!z.sT.active && !z.sI.active) return dual_after_search(z, s, out);
-  z.stage = D2_SEARCH;
+  z.stage = SZ_SEARCH;
   z.act2[0] = true; z.act2[1] = false; z.i_chain = 0;
   if (z.sT.active) {
     z.x2[0] = z.sT.x;
@@ -865,81 +982,23 @@ WVA_HD bool dual_schedule(SizerLane& z, const SysView& s, const CandView& out) {
   return true;
 }
 
-WVA_HD bool dual_begin(SizerLane& z, const SysView& s, const CandView& out) {
-  z.sT.enabled = z.sT.target > 0.0f; z.sI.enabled = z.sI.target > 0.0f;
-  z.sT.active = z.sT.enabled; z.sI.active = z.sI.enabled;
-  z.sT.result = z.m.lambda_max; z.sI.result = z.m.lambda_max;
-  z.sT.iter = z.sI.iter = 0;
-  if (z.sT.enabled || z.sI.enabled) {
-    if (z.m.lambda_min > z.m.lambda_max) { lane_fail(z, s, out); return false; }   // utils.go:29-31
-    z.stage = D2_ENDS;
-    z.x2[0] = z.m.lambda_min; z.x2[1] = z.m.lambda_max; z.act2[0] = z.act2[1] = true;
-    z.solves += 2;
-    return true;
-  }
-  return dual_after_search(z, s, out);
-}
-
 // st[c] = statistics of the solve at z.x2[c] (valid where z.act2[c]); n_states = states visited by the round
 WVA_HD bool dual_on_solve(SizerLane& z, const SysView& s, const CandView& out, const SolveStats* st, int n_states) {
   z.states += n_states;
+  if (z.stage == SZ_FINAL1 || z.stage == SZ_FINAL2) return dual_final(z, s, out, st[0]);
   const PairModel& m = z.m;
-  float pf[2], dec[2], ttft[2];
-  for (int c = 0; c < 2; c++) {
-    pf[c] = prefill_time(m, st[c].avgNumInServers);
-    dec[c] = f_div(f_sub(st[c].avgServTime, pf[c]), m.out_tok);
-    ttft[c] = f_add(f_add(st[c].avgWaitTime, pf[c]), dec[c]);
-  }
-  if (z.stage == D2_ENDS) {
-    bool infeasible = false;
-    for (int k = 0; k < 2; k++) {
-      Search& q = k ? z.sI : z.sT;
-      if (!q.active) continue;
-      const float y_lo = k ? dec[0] : ttft[0], y_hi = k ? dec[1] : ttft[1];
-      if (within_tolerance(y_lo, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_min; q.active = false; continue; }
-      if (within_tolerance(y_hi, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_max; q.active = false; continue; }
-      q.increasing = y_lo < y_hi;
-      if ((q.increasing && q.target < y_lo) || (!q.increasing && q.target > y_lo)) { infeasible = true; q.active = false; continue; }
-      if ((q.increasing && q.target > y_hi) || (!q.increasing && q.target < y_hi)) { q.result = m.lambda_max; q.active = false; continue; }
-      q.lo = m.lambda_min; q.hi = m.lambda_max; q.iter = 0;
-      q.x = f_mul(0.5f, f_add(q.lo, q.hi));
+  float ttft[2], itl[2], pf;
+  for (int c = 0; c < 2; c++) eval_values(m, st[c], &ttft[c], &itl[c], &pf);
+  if (z.stage == SZ_LO) {
+    if ((z.sT.active && !search_bracket(z.sT, m, ttft[0], ttft[1])) || (z.sI.active && !search_bracket(z.sI, m, itl[0], itl[1]))) {
+      lane_fail(z, s, out);
+      return false;
     }
-    if (infeasible) { lane_fail(z, s, out); return false; }
-    return dual_schedule(z, s, out);
+  } else {
+    if (z.sT.active) search_consume(z.sT, z.x2[0], ttft[0]);
+    if (z.sI.active) search_consume(z.sI, z.x2[z.i_chain], itl[z.i_chain]);
   }
-  if (z.stage == D2_SEARCH) {
-    const bool t_was = z.sT.active, i_was = z.sI.active;
-    if (t_was) search_consume(z.sT, z.x2[0], ttft[0]);
-    if (i_was) search_consume(z.sI, z.x2[z.i_chain], dec[z.i_chain]);
-    return dual_schedule(z, s, out);
-  }
-  if (z.stage == D2_FINAL1) {
-    z.rate_star = f_mul(st[0].throughput, 1000.0f);                                     // allocation.go:123
-    long long nr = go_int_ceil(d_div((double)z.total_rate, (double)z.rate_star));       // :132
-    if (nr < (long long)z.min_replicas) nr = z.min_replicas;
-    z.num_replicas = nr;
-    long long tot = (long long)((unsigned long long)z.n_inst * (unsigned long long)nr);
-    z.cost = f_mul(z.acc_cost, (float)tot);
-    float rate = f_div(z.total_rate, (float)nr);
-    if (!analyze_admits(m, rate)) { lane_fail(z, s, out); return false; }
-    z.stage = D2_FINAL2;
-    z.x2[0] = f_div(rate, 1000.0f); z.act2[0] = true; z.act2[1] = false;
-    z.solves++;
-    return true;
-  }
-  Alloc a;                                                                              // allocation.go:146-153
-  a.state = ALLOC_ACC;
-  a.num_replicas = z.num_replicas;
-  a.batch_size = m.N;
-  a.cost = z.cost;
-  a.itl = dec[0];
-  a.ttft = f_add(st[0].avgWaitTime, pf[0]);
-  float rho = f_div(st[0].avgNumInServers, (float)m.N);
-  a.rho = fminf(fmaxf(rho, 0.0f), 1.0f);
-  a.max_arrv = f_div(z.rate_star, 1000.0f);
-  a.value = transition_penalty(s.srv_cur_acc[z.srv], s.srv_cur_replicas[z.srv], s.srv_cur_cost[z.srv], a, z.acc);
-  store_candidate(out, (size_t)z.srv * s.n_acc + z.acc, a, z.solves);
-  return false;
+  return dual_schedule(z, s, out);
 }
 
 // ---- speculative split driver: ONE search per lane, two chains per round -------------------------------
@@ -951,12 +1010,7 @@ WVA_HD bool dual_on_solve(SizerLane& z, const SysView& s, const CandView& out, c
 // walk consumes y0 as the reference does and consumes y1 only if the next x is bit-identical to the point
 // chain 1 evaluated.  A wrong guess wastes one chain, never changes a decision.  Results are bit-identical to
 // the sequential search; a correct guess halves the rounds on the critical path (E7 with a 2-leaf tree).
-WVA_HD bool spec2_after_search(SizerLane& z, const SysView& s, const CandView& out) {
-  if (z.split >= 0 && !z.merged) { z.stage = SZ_PUBLISH; return true; }   // publish; the second finisher goes on
-  if (!dual_after_search(z, s, out)) return false;
-  z.stage = SZ_FINAL1;
-  return true;
-}
+// Items end with dual_final, as whole pairs do.
 
 // the half BinarySearch keeps if f(x) equals the interpolated value: true = [lo, x]
 WVA_HD bool spec2_predict_left(const Search& q) {
@@ -978,22 +1032,6 @@ WVA_HD bool spec2_schedule(SizerLane& z, const SysView& s, const CandView& out) 
   return true;
 }
 
-WVA_HD bool spec2_begin(SizerLane& z, const SysView& s, const CandView& out) {
-  z.sT.enabled = z.sT.target > 0.0f && z.split != 1;
-  z.sI.enabled = z.sI.target > 0.0f && z.split != 0;
-  z.sT.active = z.sT.enabled; z.sI.active = z.sI.enabled;
-  z.sT.result = z.m.lambda_max; z.sI.result = z.m.lambda_max;
-  z.sT.iter = z.sI.iter = 0;
-  if (z.sT.enabled || z.sI.enabled) {
-    if (z.m.lambda_min > z.m.lambda_max) return search_fail(z, s, out);   // utils.go:29-31
-    z.stage = SZ_LO;
-    z.x2[0] = z.m.lambda_min; z.x2[1] = z.m.lambda_max; z.act2[0] = z.act2[1] = true;
-    z.solves += 2;
-    return true;
-  }
-  return spec2_after_search(z, s, out);
-}
-
 // one consumed evaluation; keeps (y_lo, y_hi) = f at the bounds
 WVA_HD void spec2_consume(Search& q, float x, float y) {
   const bool left = (q.increasing && q.target < y) || (!q.increasing && q.target > y);
@@ -1004,43 +1042,22 @@ WVA_HD void spec2_consume(Search& q, float x, float y) {
 // st[c] = statistics of the solve at z.x2[c] (valid where z.act2[c])
 WVA_HD bool spec2_on_solve(SizerLane& z, const SysView& s, const CandView& out, const SolveStats* st, int n_states) {
   z.states += n_states;
+  if (z.stage == SZ_FINAL1 || z.stage == SZ_FINAL2) return dual_final(z, s, out, st[0]);
   const PairModel& m = z.m;
-  if (z.stage == SZ_LO || z.stage == SZ_SEARCH) {
-    Search& q = z.split == 1 ? z.sI : z.sT;
-    float y[2];
-    for (int c = 0; c < 2; c++) {
-      float pf = prefill_time(m, st[c].avgNumInServers);
-      float dec = f_div(f_sub(st[c].avgServTime, pf), m.out_tok);
-      y[c] = z.split == 1 ? dec : f_add(f_add(st[c].avgWaitTime, pf), dec);
-    }
-    if (z.stage == SZ_LO) {   // both end points (utils.go:33-57)
-      if (q.active) {
-        if (within_tolerance(y[0], q.target, WVA_BS_EPSILON)) { q.result = m.lambda_min; q.active = false; }
-        else if (within_tolerance(y[1], q.target, WVA_BS_EPSILON)) { q.result = m.lambda_max; q.active = false; }
-        else {
-          q.increasing = y[0] < y[1];
-          if ((q.increasing && q.target < y[0]) || (!q.increasing && q.target > y[0])) return search_fail(z, s, out);
-          if ((q.increasing && q.target > y[1]) || (!q.increasing && q.target < y[1])) { q.result = m.lambda_max; q.active = false; }
-          else {
-            q.lo = m.lambda_min; q.hi = m.lambda_max; q.iter = 0; q.y_lo = y[0]; q.y_hi = y[1];
-            q.x = f_mul(0.5f, f_add(q.lo, q.hi));
-          }
-        }
-      }
-      return spec2_schedule(z, s, out);
-    }
+  Search& q = z.split == 1 ? z.sI : z.sT;
+  float y[2];
+  for (int c = 0; c < 2; c++) {
+    float ttft, itl, pf;
+    eval_values(m, st[c], &ttft, &itl, &pf);
+    y[c] = z.split == 1 ? itl : ttft;
+  }
+  if (z.stage == SZ_LO) {
+    if (q.active && !search_bracket(q, m, y[0], y[1])) return search_fail(z, s, out);
+  } else {
     spec2_consume(q, z.x2[0], y[0]);
     if (q.active && z.act2[1] && q.x == z.x2[1]) spec2_consume(q, z.x2[1], y[1]);
-    return spec2_schedule(z, s, out);
   }
-  if (z.stage == SZ_FINAL1) {
-    z.stage = D2_FINAL1;
-    if (!dual_on_solve(z, s, out, st, 0)) return false;
-    z.stage = SZ_FINAL2;
-    return true;
-  }
-  z.stage = D2_FINAL2;
-  return dual_on_solve(z, s, out, st, 0);
+  return spec2_schedule(z, s, out);
 }
 
 // ---- speculative bisection (used by the warp-per-pair sizer; see sizer_warp_kernel.cuh) ----
@@ -1085,36 +1102,22 @@ WVA_HD void spec_walk(Search& q, int depth, GetY get_y) {
 WVA_HD bool sizer_on_solve(SizerLane& z, const SysView& s, const CandView& out, const SolveStats& st) {
   z.states += z.c.states;
   const PairModel& m = z.m;
-  // EvalTTFT / EvalITL / Analyze share these (queueanalyzer.go:143-149,289-292,304-305)
-  float pf = prefill_time(m, st.avgNumInServers);
-  float dec = f_div(f_sub(st.avgServTime, pf), m.out_tok);
-  float ttft_eval = f_add(f_add(st.avgWaitTime, pf), dec);
+  float ttft, itl, pf;
+  eval_values(m, st, &ttft, &itl, &pf);
   if (z.stage == SZ_LO) {
-    z.sT.y_lo = ttft_eval; z.sI.y_lo = dec;
-    if (z.sT.active && within_tolerance(ttft_eval, z.sT.target, WVA_BS_EPSILON)) { z.sT.result = m.lambda_min; z.sT.active = false; }
-    if (z.sI.active && within_tolerance(dec, z.sI.target, WVA_BS_EPSILON)) { z.sI.result = m.lambda_min; z.sI.active = false; }
+    if (z.sT.active) search_lo(z.sT, m, ttft);
+    if (z.sI.active) search_lo(z.sI, m, itl);
     if (z.sT.active || z.sI.active) { z.stage = SZ_HI; lane_start_solve(z, m.lambda_max); return true; }
     return sizer_after_search(z, s, out);
   }
   if (z.stage == SZ_HI) {
-    bool infeasible = false;
-    for (int k = 0; k < 2; k++) {
-      Search& q = k ? z.sI : z.sT;
-      if (!q.active) continue;
-      float y_hi = k ? dec : ttft_eval;
-      if (within_tolerance(y_hi, q.target, WVA_BS_EPSILON)) { q.result = m.lambda_max; q.active = false; continue; }
-      q.increasing = q.y_lo < y_hi;
-      if ((q.increasing && q.target < q.y_lo) || (!q.increasing && q.target > q.y_lo)) { infeasible = true; q.active = false; continue; }  // ind = -1
-      if ((q.increasing && q.target > y_hi) || (!q.increasing && q.target < y_hi)) { q.result = m.lambda_max; q.active = false; continue; }  // ind = +1
-      q.lo = m.lambda_min; q.hi = m.lambda_max; q.iter = 0;
-      q.x = f_mul(0.5f, f_add(q.lo, q.hi));
-    }
-    if (infeasible) return search_fail(z, s, out);   // "target is below the bounded region"
+    if ((z.sT.active && !search_hi(z.sT, m, ttft)) || (z.sI.active && !search_hi(z.sI, m, itl)))
+      return search_fail(z, s, out);   // "target is below the bounded region"
     z.stage = SZ_SEARCH;
   } else if (z.stage == SZ_SEARCH) {
     float x = z.cur_x;
-    if (z.sT.active && z.sT.x == x) search_consume(z.sT, x, ttft_eval);
-    if (z.sI.active && z.sI.x == x) search_consume(z.sI, x, dec);
+    if (z.sT.active && z.sT.x == x) search_consume(z.sT, x, ttft);
+    if (z.sI.active && z.sI.x == x) search_consume(z.sI, x, itl);
   }
   if (z.stage == SZ_SEARCH) {
     if (z.sT.active) { lane_start_solve(z, z.sT.x); return true; }
@@ -1122,32 +1125,13 @@ WVA_HD bool sizer_on_solve(SizerLane& z, const SysView& s, const CandView& out, 
     return sizer_after_search(z, s, out);
   }
   if (z.stage == SZ_FINAL1) {
-    // Size() -> metrics.Throughput; allocation.go:123-145
-    z.rate_star = f_mul(st.throughput, 1000.0f);
-    long long nr = go_int_ceil(d_div((double)z.total_rate, (double)z.rate_star));
-    if (nr < (long long)z.min_replicas) nr = z.min_replicas;
-    z.num_replicas = nr;
-    long long tot = (long long)((unsigned long long)z.n_inst * (unsigned long long)nr);
-    z.cost = f_mul(z.acc_cost, (float)tot);
-    float rate = f_div(z.total_rate, (float)nr);
-    if (!analyze_admits(m, rate)) { lane_fail(z, s, out); return false; }
+    float x;
+    if (!alloc_replicas(z, st.throughput, x)) { lane_fail(z, s, out); return false; }
     z.stage = SZ_FINAL2;
-    lane_start_solve(z, f_div(rate, 1000.0f));
+    lane_start_solve(z, x);
     return true;
   }
-  // SZ_FINAL2: allocation.go:146-153
-  Alloc a;
-  a.state = ALLOC_ACC;
-  a.num_replicas = z.num_replicas;
-  a.batch_size = m.N;
-  a.cost = z.cost;
-  a.itl = dec;
-  a.ttft = f_add(st.avgWaitTime, pf);
-  float rho = f_div(st.avgNumInServers, (float)m.N);
-  rho = fminf(fmaxf(rho, 0.0f), 1.0f);
-  a.rho = rho;
-  a.max_arrv = f_div(z.rate_star, 1000.0f);
-  a.value = transition_penalty(s.srv_cur_acc[z.srv], s.srv_cur_replicas[z.srv], s.srv_cur_cost[z.srv], a, z.acc);
+  const Alloc a = alloc_final(z, s, st, itl, pf);   // SZ_FINAL2
   store_candidate(out, (size_t)z.srv * s.n_acc + z.acc, a, z.solves);
   return false;
 }

@@ -37,11 +37,6 @@ static SolveStats host_solve(const PairModel& m, float x, bool* ovf) {
   *ovf = c.phase == CH_OVERFLOW;
   return st;
 }
-static void host_eval(const PairModel& m, const SolveStats& st, float* ttft, float* itl, float* pf) {
-  *pf = prefill_time(m, st.avgNumInServers);
-  *itl = f_div(f_sub(st.avgServTime, *pf), m.out_tok);
-  *ttft = f_add(f_add(st.avgWaitTime, *pf), *itl);
-}
 
 // System.Calculate through the SPECULATIVE bisection of sizer_warp_kernel.cuh, replayed lane by lane
 // (tests spec_node_x / spec_walk and the round structure against the oracle).
@@ -61,35 +56,25 @@ extern "C" int emul_calculate_spec(const wva_system* sys, wva_candidates* out) {
       model_finish(z.m, tab.data(), 1);
       PairModel& m = z.m;
       size_t idx = (size_t)srv * s.n_acc + acc;
-      Alloc fail; fail.state = ALLOC_NONE; fail.num_replicas = 0; fail.batch_size = 0;
-      fail.cost = fail.value = fail.itl = fail.ttft = fail.rho = fail.max_arrv = 0.0f;
       bool failed = false, ovf = false;
-      Search sT, sI;
-      sT.target = z.sT.target; sI.target = z.sI.target;
-      sT.enabled = sT.target > 0; sI.enabled = sI.target > 0;
-      sT.active = sT.enabled; sI.active = sI.enabled;
-      sT.result = sI.result = m.lambda_max; sT.iter = sI.iter = 0;
+      Search& sT = z.sT;
+      Search& sI = z.sI;
       float yt[32], yi[32], pf;
-      if (sT.enabled || sI.enabled) {
+      if (searches_begin(z)) {
         if (m.lambda_min > m.lambda_max) failed = true;
         else {
           for (int lane = 0; lane < 17; lane++) {
             float x = lane == 0 ? m.lambda_min : lane == 1 ? m.lambda_max
                       : spec_node_x(m.lambda_min, m.lambda_max, lane - 1, spec_depth_of(lane - 1));
             SolveStats st = host_solve(m, x, &ovf);
-            host_eval(m, st, &yt[lane], &yi[lane], &pf);
+            eval_values(m, st, &yt[lane], &yi[lane], &pf);
           }
           for (int k = 0; k < 2; k++) {
             Search& q = k ? sI : sT;
             if (!q.active) continue;
             float* y = k ? yi : yt;
-            if (within_tolerance(y[0], q.target, WVA_BS_EPSILON)) { q.result = m.lambda_min; q.active = false; continue; }
-            if (within_tolerance(y[1], q.target, WVA_BS_EPSILON)) { q.result = m.lambda_max; q.active = false; continue; }
-            q.increasing = y[0] < y[1];
-            if ((q.increasing && q.target < y[0]) || (!q.increasing && q.target > y[0])) { failed = true; q.active = false; continue; }
-            if ((q.increasing && q.target > y[1]) || (!q.increasing && q.target < y[1])) { q.result = m.lambda_max; q.active = false; continue; }
-            q.lo = m.lambda_min; q.hi = m.lambda_max; q.iter = 0; q.x = f_mul(0.5f, f_add(q.lo, q.hi));
-            spec_walk(q, 4, [&](int node) { return y[node + 1]; });
+            if (!search_bracket(q, m, y[0], y[1])) failed = true;
+            else if (q.active) spec_walk(q, 4, [&](int node) { return y[node + 1]; });
           }
           while (!failed && (sT.active || sI.active)) {
             bool both = sT.active && sI.active;
@@ -101,7 +86,7 @@ extern "C" int emul_calculate_spec(const wva_system* sys, wva_candidates* out) {
               const Search& mq = isI ? sI : sT;
               float x = spec_node_x(mq.lo, mq.hi, node, spec_depth_of(node));
               SolveStats st = host_solve(m, x, &ovf);
-              host_eval(m, st, &yt[lane], &yi[lane], &pf);
+              eval_values(m, st, &yt[lane], &yi[lane], &pf);
             }
             if (both) { spec_walk(sT, D, [&](int nd) { return yt[nd - 1]; }); spec_walk(sI, D, [&](int nd) { return yi[16 + nd - 1]; }); }
             else if (sT.active) spec_walk(sT, D, [&](int nd) { return yt[nd - 1]; });
@@ -109,31 +94,15 @@ extern "C" int emul_calculate_spec(const wva_system* sys, wva_candidates* out) {
           }
         }
       }
-      Alloc a = fail;
-      if (!failed) {
-        float l_tps = m.lambda_max;
-        if (z.slo_tps > 0) l_tps = f_mul(m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));
-        float lambda = fminf(fminf(sT.result, sI.result), l_tps);
-        float rr = f_mul(lambda, 1000.0f);
-        if (analyze_admits(m, rr)) {
-          SolveStats st = host_solve(m, f_div(rr, 1000.0f), &ovf);
-          float rate_star = f_mul(st.throughput, 1000.0f);
-          long long nr = go_int_ceil(d_div((double)z.total_rate, (double)rate_star));
-          if (nr < z.min_replicas) nr = z.min_replicas;
-          long long tot = (long long)((unsigned long long)z.n_inst * (unsigned long long)nr);
-          float cost = f_mul(z.acc_cost, (float)tot);
-          float rate = f_div(z.total_rate, (float)nr);
-          if (analyze_admits(m, rate)) {
-            st = host_solve(m, f_div(rate, 1000.0f), &ovf);
-            float t, i2;
-            host_eval(m, st, &t, &i2, &pf);
-            a.state = ALLOC_ACC; a.num_replicas = nr; a.batch_size = m.N; a.cost = cost; a.itl = i2;
-            a.ttft = f_add(st.avgWaitTime, pf);
-            float rho = f_div(st.avgNumInServers, (float)m.N);
-            a.rho = fminf(fmaxf(rho, 0.0f), 1.0f);
-            a.max_arrv = f_div(rate_star, 1000.0f);
-            a.value = transition_penalty(s.srv_cur_acc[srv], s.srv_cur_replicas[srv], s.srv_cur_cost[srv], a, acc);
-          }
+      Alloc a = alloc_none();
+      float x;
+      if (!failed && size_lambda(z, x)) {
+        SolveStats st = host_solve(m, x, &ovf);
+        if (alloc_replicas(z, st.throughput, x)) {
+          st = host_solve(m, x, &ovf);
+          float t, i2;
+          eval_values(m, st, &t, &i2, &pf);
+          a = alloc_final(z, s, st, i2, pf);
         }
       }
       store_candidate(o, idx, a, 0);
@@ -253,7 +222,7 @@ extern "C" int emul_probe_debug(const wva_system* sys, int item) {
     ProbeEval e = probe_eval(m, nullptr, x), e2 = e;
     bool ovf; SolveStats st; float t, i, pf; 
     std::vector<float> tab(m.N); model_fill_table(m, tab.data(), 1, 0, 1); PairModel mm = m; model_finish(mm, tab.data(), 1);
-    st = host_solve(mm, x, &ovf); host_eval(mm, st, &t, &i, &pf);
+    st = host_solve(mm, x, &ovf); eval_values(mm, st, &t, &i, &pf);
     printf("  x %g probe ttft %g itl %g len %d len54 %d | exact ttft %g itl %g\n", x, e.ttft, e.itl, e.len, e2.len, t, i);
   }
   return 0;

@@ -274,7 +274,7 @@ int emul_grid_deferred(const wva_system* sys, int R, float thr, uint8_t* ok, flo
           if (ovf) { counts[3]++; continue; }
         }
         float pf, dec, avg_ttft;
-        host_eval(m, st, &avg_ttft, &dec, &pf);
+        eval_values(m, st, &avg_ttft, &dec, &pf);
         float rh = f_div(st.avgNumInServers, (float)m.N);
         rh = fminf(fmaxf(rh, 0.0f), 1.0f);
         ok[o] = 1;
