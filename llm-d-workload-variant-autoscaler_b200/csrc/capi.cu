@@ -62,11 +62,127 @@ struct PinBuf {  // growable pinned host staging
   void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
 
-// bump allocator over one arena: every sub-array 256-byte aligned
+// ------------------------------------------------------------------ column lists
+// Every struct-of-arrays of the C-ABI is declared once, in the order its arena is laid out: X(field, count, flags).  The
+// public struct (include/wva_b200.h) and its device view share the field names, so one visitor per list walks any of
+// them: each_<list>(n, f, s...) calls f(count, flags, s.field...) for every column.  Element sizes come from the fields.
+// Counts are written over the extents `n`; over the entities BEFORE a block (servers before a rank's block, models /
+// variants / replicas before a group member's block) a column's count is its offset to that block.
+struct Ext { size_t A = 0, T = 0, M = 0, S = 0, V = 0, P = 0, R = 0; };   // P: pairs or replicas, R: grid levels
+enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL too
+       COL_DETAIL = 2 };  // V1 saturation analysis field: written only by a detail run
+
+#define SYS_COLS(X)                                                                                                    \
+  X(acc_cost, n.A, 0) X(acc_multiplicity, n.A, 0) X(acc_type, n.A, 0) X(type_count, n.T, 0)                            \
+  X(perf_alpha, n.M * n.A, 0) X(perf_beta, n.M * n.A, 0) X(perf_gamma, n.M * n.A, 0) X(perf_max_batch, n.M * n.A, 0)  \
+  X(perf_at_tokens, n.M * n.A, 0) X(perf_acc_count, n.M * n.A, 0) X(perf_present, n.M * n.A, 0)                        \
+  X(srv_model, n.S, 0) X(srv_priority, n.S, 0) X(srv_min_replicas, n.S, 0) X(srv_max_batch, n.S, 0)                    \
+  X(srv_keep_acc, n.S, 0) X(srv_target_present, n.S, 0) X(srv_slo_ttft, n.S, 0) X(srv_slo_itl, n.S, 0)                \
+  X(srv_slo_tps, n.S, 0) X(srv_arrival, n.S, 0) X(srv_in_tokens, n.S, 0) X(srv_out_tokens, n.S, 0)                     \
+  X(srv_cur_acc, n.S, 0) X(srv_cur_replicas, n.S, 0) X(srv_cur_cost, n.S, 0)
+#define CAND_COLS(X)                                                                                                   \
+  X(state, n.P, 0) X(num_replicas, n.P, 0) X(batch_size, n.P, 0) X(cost, n.P, 0) X(value, n.P, 0) X(itl, n.P, 0)      \
+  X(ttft, n.P, 0) X(rho, n.P, 0) X(max_arrv_rate, n.P, 0) X(n_solves, n.P, COL_OPT)
+#define SOL_COLS(X)                                                                                                    \
+  X(state, n.S, 0) X(acc, n.S, 0) X(num_replicas, n.S, 0) X(batch_size, n.S, 0) X(cost, n.S, 0) X(value, n.S, 0)      \
+  X(itl, n.S, 0) X(ttft, n.S, 0) X(rho, n.S, 0) X(max_arrv_rate, n.S, 0)
+// the variant and model columns of wva_saturation_in, which the ingest column arena lays out in the same order
+#define SAT_IN_SHARED_COLS(X)                                                                                          \
+  X(var_cost, n.V, 0) X(var_current, n.V, 0) X(var_desired, n.V, 0) X(var_pending, n.V, 0)                             \
+  X(cfg_kv_threshold, n.M, 0) X(cfg_queue_threshold, n.M, 0) X(cfg_kv_trigger, n.M, 0) X(cfg_queue_trigger, n.M, 0)
+#define SAT_IN_COLS(X)                                                                                                 \
+  X(model_variant_off, n.M + 1, 0) X(variant_replica_off, n.V + 1, 0) X(rep_kv, n.P, 0) X(rep_queue, n.P, 0)           \
+  X(var_cost, n.V, 0) X(var_current, n.V, 0) X(var_desired, n.V, 0) X(var_pending, n.V, 0)                             \
+  X(var_has_state, n.V, COL_OPT)                                                                                       \
+  X(cfg_kv_threshold, n.M, 0) X(cfg_queue_threshold, n.M, 0) X(cfg_kv_trigger, n.M, 0) X(cfg_queue_trigger, n.M, 0)
+#define SAT_OUT_COLS(X)                                                                                                \
+  X(var_target, n.V, 0) X(var_replica_count, n.V, COL_DETAIL) X(var_non_saturated, n.V, COL_DETAIL)                    \
+  X(var_max_kv, n.V, COL_DETAIL) X(var_max_queue, n.V, COL_DETAIL) X(var_avg_spare_kv, n.V, COL_DETAIL)                \
+  X(var_avg_spare_queue, n.V, COL_DETAIL) X(rep_saturated, n.P, COL_DETAIL) X(mod_total_replicas, n.M, COL_DETAIL)     \
+  X(mod_non_saturated, n.M, COL_DETAIL) X(mod_avg_spare_kv, n.M, COL_DETAIL) X(mod_avg_spare_queue, n.M, COL_DETAIL)   \
+  X(mod_flags, n.M, 0)
+#define V2_IN_COLS(X)                                                                                                  \
+  X(model_variant_off, n.M + 1, 0) X(variant_replica_off, n.V + 1, 0) X(rep_total_kv_tokens, n.P, 0)                   \
+  X(rep_tokens_in_use, n.P, 0) X(rep_queue_length, n.P, 0) X(rep_avg_input_tokens, n.P, 0)                             \
+  X(rep_avg_output_tokens, n.P, 0) X(rep_prefix_hit_rate, n.P, 0) X(rep_k2, n.P, 0) X(rep_slice_order, n.P, COL_OPT)   \
+  X(var_current, n.V, 0) X(var_pending, n.V, 0) X(var_fallback_capacity, n.V, 0) X(cfg_kv_threshold, n.M, 0)          \
+  X(cfg_scale_up_threshold, n.M, 0) X(cfg_scale_down_boundary, n.M, 0) X(sched_queue_size, n.M, COL_OPT)               \
+  X(sched_queue_bytes, n.M, COL_OPT)
+#define V2_OUT_COLS(X)                                                                                                 \
+  X(rep_k1, n.P, 0) X(rep_effective, n.P, 0) X(rep_demand, n.P, 0) X(rep_saturated, n.P, 0) X(var_ready, n.V, 0)      \
+  X(var_per_replica_capacity, n.V, 0) X(var_total_capacity, n.V, 0) X(var_total_demand, n.V, 0)                        \
+  X(var_utilization, n.V, 0) X(mod_total_supply, n.M, 0) X(mod_total_demand, n.M, 0) X(mod_utilization, n.M, 0)        \
+  X(mod_required_capacity, n.M, 0) X(mod_spare_capacity, n.M, 0)
+// the replica grid's optional outputs (wva_grid_run with full != 0)
+#define GRID_COLS(X)                                                                                                   \
+  X(ok, n.P * n.R, 0) X(ttft, n.P * n.R, 0) X(itl, n.P * n.R, 0) X(rho, n.P * n.R, 0) X(tput, n.P * n.R, 0)
+
+#define COL_VISIT_(field, count, flags) f((size_t)(count), flags, s.field...);
+#define COL_VISITOR_(name, LIST) \
+  template <class F, class... Structs> static void name(const Ext& n, F&& f, Structs&&... s) { LIST(COL_VISIT_) }
+COL_VISITOR_(each_sys, SYS_COLS)
+COL_VISITOR_(each_cand, CAND_COLS)
+COL_VISITOR_(each_sol, SOL_COLS)
+COL_VISITOR_(each_sat_shared, SAT_IN_SHARED_COLS)
+COL_VISITOR_(each_sat_in, SAT_IN_COLS)
+COL_VISITOR_(each_sat_out, SAT_OUT_COLS)
+COL_VISITOR_(each_v2_in, V2_IN_COLS)
+COL_VISITOR_(each_v2_out, V2_OUT_COLS)
+COL_VISITOR_(each_grid, GRID_COLS)
+#undef COL_VISITOR_
+#undef COL_VISIT_
+
+// Column functors: f(count, flags, view field, caller's field).  They are called through the lists above, and directly
+// for the few columns that belong to one entry point only.
+
+// bump allocator over one arena: every sub-array 256-byte aligned.  As a functor it lays out the next column and, once
+// the arena has a base, points the view's field at it; a pass without a base only sizes the arena.
 struct Layout {
+  char* base = nullptr;
   size_t off = 0;
   size_t take(size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; }
+  template <class T, class... H> void operator()(size_t n, int, T*& p, H&&...) {
+    const size_t o = take(n * sizeof(T));
+    if (base) p = (T*)(base + o);
+  }
 };
+// copies the columns the caller supplied (non-NULL, not empty) into the view (H2D) or out of it (D2H); keeps the first error
+struct Copy {
+  cudaStream_t s;
+  cudaMemcpyKind kind;
+  cudaError_t e = cudaSuccess;
+  template <class T, class H> void operator()(size_t n, int, T* d, H* h) {
+    if (!h || !n || e != cudaSuccess) return;
+    const bool up = kind == cudaMemcpyHostToDevice;
+    e = cudaMemcpyAsync(up ? (void*)d : (void*)h, up ? (const void*)h : (const void*)d, n * sizeof(T), kind, s);
+  }
+};
+// lays out an input arena and copies the caller's arrays into it; an optional column the caller left NULL is NULL
+struct Upload : Layout {
+  Copy copy;
+  explicit Upload(cudaStream_t s) : copy{s, cudaMemcpyHostToDevice} {}
+  template <class T, class H> void operator()(size_t n, int flags, T*& d, H* h) {
+    const size_t o = take(n * sizeof(T));
+    if (!base) return;
+    d = (h || !(flags & COL_OPT)) ? (T*)(base + o) : nullptr;
+    copy(n, flags, d, h);
+  }
+};
+// true once a column that is not optional and not empty was left NULL by the caller
+struct Missing {
+  bool any = false;
+  template <class T, class H> void operator()(size_t n, int flags, T*, H* h) { any |= n && !h && !(flags & COL_OPT); }
+};
+
+// Sizes an arena with a pass of `lay` over a copy of `f` that has no base, reserves it, then runs `lay` over `f` with the
+// arena as its base.  Nothing is bound and nothing copied unless the reservation succeeds.
+template <class F, class Lay> static cudaError_t lay_out(DevBuf& buf, F& f, Lay&& lay) {
+  F sizing = f;
+  lay(sizing);
+  const cudaError_t e = buf.reserve(sizing.off + 256);
+  if (e == cudaSuccess) { f.base = (char*)buf.p; lay(f); }
+  return e;
+}
 
 struct GridState {   // results of the last wva_grid_run, resident in HBM
   int R = 0;
@@ -81,7 +197,6 @@ struct SatState {    // resident inputs / outputs of the saturation model
   DevBuf in, out, desc;
   SatIn vin = {};
   SatOut vout = {};
-  size_t out_bytes = 0;
 };
 
 struct wva_ctx {
@@ -129,29 +244,20 @@ struct wva_ctx {
 
 // views of the rank's block of servers: srv_* arrays and the candidate rows are plain arrays indexed by server, so a
 // block is the same struct with offset pointers and n_servers = block size (models / accelerators stay global)
+static Ext before_block(const wva_ctx* ctx) {   // the servers before the block (no models, accelerators or types)
+  Ext n;
+  n.S = (size_t)ctx->shard_lo; n.P = (size_t)ctx->shard_lo * ctx->A;
+  return n;
+}
+static const auto advance = [](size_t n, int, auto*& p) { p += n; };
 static SysView shard_sys(const wva_ctx* ctx) {
   SysView v = ctx->sys;
-  const int lo = ctx->shard_lo;
+  each_sys(before_block(ctx), advance, v);
   v.n_servers = ctx->shard_hi - ctx->shard_lo;
-  v.srv_model += lo; v.srv_priority += lo; v.srv_min_replicas += lo; v.srv_max_batch += lo; v.srv_keep_acc += lo;
-  v.srv_target_present += lo; v.srv_slo_ttft += lo; v.srv_slo_itl += lo; v.srv_slo_tps += lo; v.srv_arrival += lo;
-  v.srv_in_tokens += lo; v.srv_out_tokens += lo; v.srv_cur_acc += lo; v.srv_cur_replicas += lo; v.srv_cur_cost += lo;
   return v;
 }
-static CandView shard_cand(const wva_ctx* ctx) {
-  CandView c = ctx->cand;
-  const size_t o = (size_t)ctx->shard_lo * ctx->A;
-  c.state += o; c.num_replicas += o; c.batch_size += o; c.cost += o; c.value += o; c.itl += o; c.ttft += o; c.rho += o;
-  c.max_arrv_rate += o; c.n_solves += o;
-  return c;
-}
-static SolView shard_sol(const wva_ctx* ctx) {
-  SolView c = ctx->sol;
-  const size_t o = (size_t)ctx->shard_lo;
-  c.state += o; c.acc += o; c.num_replicas += o; c.batch_size += o; c.cost += o; c.value += o; c.itl += o; c.ttft += o;
-  c.rho += o; c.max_arrv_rate += o;
-  return c;
-}
+static CandView shard_cand(const wva_ctx* ctx) { CandView c = ctx->cand; each_cand(before_block(ctx), advance, c); return c; }
+static SolView shard_sol(const wva_ctx* ctx) { SolView o = ctx->sol; each_sol(before_block(ctx), advance, o); return o; }
 static int32_t comm_exchange_and_solve(wva_ctx* ctx);   // comm.inl
 static int32_t comm_reduce_sat_partials(wva_ctx* ctx, long long* d_partials, long long* d_all);
 static int32_t comm_agree_status(wva_ctx* ctx, int my_status, int* agreed);
@@ -237,21 +343,11 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   if (s->n_types > WVA_MAX_TYPES) { ctx->last_error = "wva_load_system: more than 64 capacity types"; return WVA_ERR_LIMIT; }
   CK(cudaSetDevice(ctx->device));
   const size_t A = s->n_acc, T = s->n_types, M = s->n_models, S = s->n_servers, MA = M * A;
-  struct Item { const void* src; size_t bytes; size_t off; };
-  Layout L;
-  std::vector<Item> items;
-  auto add = [&](const void* p, size_t bytes) { Item it{p, bytes, L.take(bytes)}; items.push_back(it); return it.off; };
-  size_t o_acc_cost = add(s->acc_cost, A * 4), o_acc_mult = add(s->acc_multiplicity, A * 4),
-         o_acc_type = add(s->acc_type, A * 4), o_type_count = add(s->type_count, T * 4);
-  size_t o_pa = add(s->perf_alpha, MA * 4), o_pb = add(s->perf_beta, MA * 4), o_pg = add(s->perf_gamma, MA * 4),
-         o_pmb = add(s->perf_max_batch, MA * 4), o_pat = add(s->perf_at_tokens, MA * 4),
-         o_pac = add(s->perf_acc_count, MA * 4), o_pp = add(s->perf_present, MA);
-  size_t o_sm = add(s->srv_model, S * 4), o_sp = add(s->srv_priority, S * 4), o_smr = add(s->srv_min_replicas, S * 4),
-         o_smb = add(s->srv_max_batch, S * 4), o_sk = add(s->srv_keep_acc, S), o_stp = add(s->srv_target_present, S),
-         o_st = add(s->srv_slo_ttft, S * 4), o_si = add(s->srv_slo_itl, S * 4), o_sps = add(s->srv_slo_tps, S * 4),
-         o_sa = add(s->srv_arrival, S * 4), o_sin = add(s->srv_in_tokens, S * 4), o_sout = add(s->srv_out_tokens, S * 4),
-         o_sca = add(s->srv_cur_acc, S * 4), o_scr = add(s->srv_cur_replicas, S * 4), o_scc = add(s->srv_cur_cost, S * 4);
-  for (auto& it : items) if (it.bytes && !it.src) { ctx->last_error = "wva_load_system: a required array is NULL"; return WVA_ERR_ARG; }
+  Ext n;
+  n.A = A; n.T = T; n.M = M; n.S = S;
+  Missing miss;
+  each_sys(n, miss, ctx->sys, *s);
+  if (miss.any) { ctx->last_error = "wva_load_system: a required array is NULL"; return WVA_ERR_ARG; }
   // validate indices the kernels dereference (after the NULL checks above)
   for (size_t a = 0; a < A; a++)
     if (s->acc_type[a] < 0 || s->acc_type[a] >= (int)T) { ctx->last_error = "wva_load_system: acc_type out of range"; return WVA_ERR_ARG; }
@@ -270,28 +366,20 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
       return WVA_ERR_ARG;
     }
   }
+  // one H2D copy of the whole arena, staged in pinned memory at the arena's offsets
+  Layout L;
+  each_sys(n, L, ctx->sys);
   const size_t total = L.off + 256;
   CK(ctx->stage_in.reserve(total));
   CK(ctx->sys_arena.reserve(total));
   char* h = (char*)ctx->stage_in.p;
-  for (auto& it : items) if (it.bytes) memcpy(h + it.off, it.src, it.bytes);
+  L = Layout{(char*)ctx->sys_arena.p};
+  each_sys(n, [&](size_t c, int, auto*& d, auto* src) { if (c) memcpy(h + L.off, src, c * sizeof(*d)); L(c, 0, d); }, ctx->sys, *s);
   CK(cudaEventRecord(ctx->ev[0], ctx->stream));
   CK(cudaMemcpyAsync(ctx->sys_arena.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaEventRecord(ctx->ev[1], ctx->stream));
-  char* d = (char*)ctx->sys_arena.p;
   SysView& v = ctx->sys;
   v.n_acc = (int)A; v.n_types = (int)T; v.n_models = (int)M; v.n_servers = (int)S;
-  v.acc_cost = (const float*)(d + o_acc_cost); v.acc_multiplicity = (const int*)(d + o_acc_mult);
-  v.acc_type = (const int*)(d + o_acc_type); v.type_count = (const int*)(d + o_type_count);
-  v.perf_alpha = (const float*)(d + o_pa); v.perf_beta = (const float*)(d + o_pb); v.perf_gamma = (const float*)(d + o_pg);
-  v.perf_max_batch = (const int*)(d + o_pmb); v.perf_at_tokens = (const int*)(d + o_pat);
-  v.perf_acc_count = (const int*)(d + o_pac); v.perf_present = (const unsigned char*)(d + o_pp);
-  v.srv_model = (const int*)(d + o_sm); v.srv_priority = (const int*)(d + o_sp);
-  v.srv_min_replicas = (const int*)(d + o_smr); v.srv_max_batch = (const int*)(d + o_smb);
-  v.srv_keep_acc = (const unsigned char*)(d + o_sk); v.srv_target_present = (const unsigned char*)(d + o_stp);
-  v.srv_slo_ttft = (const float*)(d + o_st); v.srv_slo_itl = (const float*)(d + o_si); v.srv_slo_tps = (const float*)(d + o_sps);
-  v.srv_arrival = (const float*)(d + o_sa); v.srv_in_tokens = (const int*)(d + o_sin); v.srv_out_tokens = (const int*)(d + o_sout);
-  v.srv_cur_acc = (const int*)(d + o_sca); v.srv_cur_replicas = (const int*)(d + o_scr); v.srv_cur_cost = (const float*)(d + o_scc);
   ctx->A = (int)A; ctx->T = (int)T; ctx->M = (int)M; ctx->S = (int)S;
   ctx->unlimited = s->unlimited; ctx->delayed = s->delayed_best_effort; ctx->policy = s->saturation_policy;
 
@@ -301,35 +389,13 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   ctx->shard_lo = ctx->world > 1 ? (int)std::min(S, (size_t)ctx->rank * ctx->shard_rows) : 0;
   ctx->shard_hi = ctx->world > 1 ? (int)std::min(S, (size_t)(ctx->rank + 1) * ctx->shard_rows) : (int)S;
   const size_t S_pad = ctx->world > 1 ? (size_t)ctx->shard_rows * ctx->world : S;
-  const size_t P = S_pad * A;
-  {
-    Layout C;
-    size_t o_state = C.take(P), o_nr = C.take(P * 4), o_bs = C.take(P * 4), o_cost = C.take(P * 4), o_val = C.take(P * 4),
-           o_itl = C.take(P * 4), o_ttft = C.take(P * 4), o_rho = C.take(P * 4), o_mar = C.take(P * 4), o_ns = C.take(P * 4);
-    CK(ctx->cand_arena.reserve(C.off + 256));
-    char* c = (char*)ctx->cand_arena.p;
-    CandView& cv = ctx->cand;
-    cv.state = (unsigned char*)(c + o_state); cv.num_replicas = (int*)(c + o_nr); cv.batch_size = (int*)(c + o_bs);
-    cv.cost = (float*)(c + o_cost); cv.value = (float*)(c + o_val); cv.itl = (float*)(c + o_itl);
-    cv.ttft = (float*)(c + o_ttft); cv.rho = (float*)(c + o_rho); cv.max_arrv_rate = (float*)(c + o_mar);
-    cv.n_solves = (int*)(c + o_ns);
-  }
-  {
-    Layout C;
-    const size_t SP = S_pad;
-    size_t o_state = C.take(SP), o_acc = C.take(SP * 4), o_nr = C.take(SP * 4), o_bs = C.take(SP * 4), o_cost = C.take(SP * 4),
-           o_val = C.take(SP * 4), o_itl = C.take(SP * 4), o_ttft = C.take(SP * 4), o_rho = C.take(SP * 4), o_mar = C.take(SP * 4),
-           o_tc = C.take(T * 8), o_tk = C.take(T * 8);
-    CK(ctx->sol_arena.reserve(C.off + 256));
-    CK(cudaMemsetAsync(ctx->sol_arena.p, 0, ctx->sol_arena.cap, ctx->stream));   // padding is copied out with the arena
-    char* c = (char*)ctx->sol_arena.p;
-    SolView& sv = ctx->sol;
-    sv.state = (unsigned char*)(c + o_state); sv.acc = (int*)(c + o_acc); sv.num_replicas = (int*)(c + o_nr);
-    sv.batch_size = (int*)(c + o_bs); sv.cost = (float*)(c + o_cost); sv.value = (float*)(c + o_val);
-    sv.itl = (float*)(c + o_itl); sv.ttft = (float*)(c + o_ttft); sv.rho = (float*)(c + o_rho);
-    sv.max_arrv_rate = (float*)(c + o_mar);
-    ctx->d_type_count = (long long*)(c + o_tc); ctx->d_type_cost = (double*)(c + o_tk);
-  }
+  Ext pad;
+  pad.S = S_pad; pad.P = S_pad * A;
+  Layout C;
+  CK(lay_out(ctx->cand_arena, C, [&](Layout& f) { each_cand(pad, f, ctx->cand); }));
+  Layout O;
+  CK(lay_out(ctx->sol_arena, O, [&](Layout& f) { each_sol(pad, f, ctx->sol); f(T, 0, ctx->d_type_count); f(T, 0, ctx->d_type_cost); }));
+  CK(cudaMemsetAsync(ctx->sol_arena.p, 0, ctx->sol_arena.cap, ctx->stream));   // padding is copied out with the arena
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
   ctx->loaded = true; ctx->calculated = false; ctx->solved = false;
@@ -685,9 +751,12 @@ int32_t wva_set_capacity(wva_ctx* ctx, const int32_t* type_count) {
 int32_t wva_set_candidates(wva_ctx* ctx, const wva_candidates* in) {
   if (!ctx || !in) return WVA_ERR_ARG;
   if (!ctx->loaded) { ctx->last_error = "wva_set_candidates before wva_load_system"; return WVA_ERR_STATE; }
-  const size_t P = (size_t)ctx->S * ctx->A;
-  if (P > 0 && (!in->state || !in->num_replicas || !in->batch_size || !in->cost || !in->value || !in->itl || !in->ttft ||
-                !in->rho || !in->max_arrv_rate)) {
+  Ext n;
+  n.P = (size_t)ctx->S * ctx->A;
+  const size_t P = n.P;
+  Missing miss;
+  each_cand(n, miss, ctx->cand, *in);
+  if (miss.any) {
     ctx->last_error = "wva_set_candidates: a required array is NULL";
     return WVA_ERR_ARG;
   }
@@ -698,16 +767,10 @@ int32_t wva_set_candidates(wva_ctx* ctx, const wva_candidates* in) {
     }
   CK(cudaSetDevice(ctx->device));
   CK(cudaEventRecord(ctx->ev[0], ctx->stream));
-  const CandView& c = ctx->cand;
-  struct { void* dst; const void* src; size_t b; } cp[] = {
-      {c.state, in->state, P}, {c.num_replicas, in->num_replicas, P * 4}, {c.batch_size, in->batch_size, P * 4},
-      {c.cost, in->cost, P * 4}, {c.value, in->value, P * 4}, {c.itl, in->itl, P * 4}, {c.ttft, in->ttft, P * 4},
-      {c.rho, in->rho, P * 4}, {c.max_arrv_rate, in->max_arrv_rate, P * 4}};
-  if (P > 0) {
-    for (auto& x : cp) CK(cudaMemcpyAsync(x.dst, x.src, x.b, cudaMemcpyHostToDevice, ctx->stream));
-    if (in->n_solves) CK(cudaMemcpyAsync(c.n_solves, in->n_solves, P * 4, cudaMemcpyHostToDevice, ctx->stream));
-    else CK(cudaMemsetAsync(c.n_solves, 0, P * 4, ctx->stream));
-  }
+  Copy up{ctx->stream, cudaMemcpyHostToDevice};
+  each_cand(n, up, ctx->cand, *in);
+  CK(up.e);
+  if (P > 0 && !in->n_solves) CK(cudaMemsetAsync(ctx->cand.n_solves, 0, P * 4, ctx->stream));
   CK(cudaEventRecord(ctx->ev[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));               // the caller's buffers are free again on return (cgo pointer rule)
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
@@ -720,16 +783,13 @@ int32_t wva_get_candidates(wva_ctx* ctx, wva_candidates* out) {
   if (!ctx || !out) return WVA_ERR_ARG;
   if (!ctx->calculated) { ctx->last_error = "wva_get_candidates before wva_calculate"; return WVA_ERR_STATE; }
   CK(cudaSetDevice(ctx->device));
-  const size_t P = (size_t)ctx->S * ctx->A;
-  if (P == 0) return WVA_OK;
+  Ext n;
+  n.P = (size_t)ctx->S * ctx->A;
+  if (n.P == 0) return WVA_OK;
   CK(cudaEventRecord(ctx->ev[6], ctx->stream));
-  const CandView& c = ctx->cand;
-  struct { void* dst; const void* src; size_t b; } cp[] = {
-      {out->state, c.state, P}, {out->num_replicas, c.num_replicas, P * 4}, {out->batch_size, c.batch_size, P * 4},
-      {out->cost, c.cost, P * 4}, {out->value, c.value, P * 4}, {out->itl, c.itl, P * 4}, {out->ttft, c.ttft, P * 4},
-      {out->rho, c.rho, P * 4}, {out->max_arrv_rate, c.max_arrv_rate, P * 4}, {out->n_solves, c.n_solves, P * 4}};
-  for (auto& x : cp)
-    if (x.dst) CK(cudaMemcpyAsync(x.dst, x.src, x.b, cudaMemcpyDeviceToHost, ctx->stream));
+  Copy down{ctx->stream, cudaMemcpyDeviceToHost};
+  each_cand(n, down, ctx->cand, *out);
+  CK(down.e);
   CK(cudaEventRecord(ctx->ev[7], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->timing.d2h_ms = elapsed(ctx, 6, 7);
@@ -752,17 +812,9 @@ int32_t wva_get_solution(wva_ctx* ctx, wva_solution* out) {
   const char* h = (const char*)ctx->stage_out.p;
   const char* d = (const char*)ctx->sol_arena.p;
   auto H = [&](const void* devp) { return h + ((const char*)devp - d); };
-  const SolView& v = ctx->sol;
-  if (out->state) memcpy(out->state, H(v.state), S);
-  if (out->acc) memcpy(out->acc, H(v.acc), S * 4);
-  if (out->num_replicas) memcpy(out->num_replicas, H(v.num_replicas), S * 4);
-  if (out->batch_size) memcpy(out->batch_size, H(v.batch_size), S * 4);
-  if (out->cost) memcpy(out->cost, H(v.cost), S * 4);
-  if (out->value) memcpy(out->value, H(v.value), S * 4);
-  if (out->itl) memcpy(out->itl, H(v.itl), S * 4);
-  if (out->ttft) memcpy(out->ttft, H(v.ttft), S * 4);
-  if (out->rho) memcpy(out->rho, H(v.rho), S * 4);
-  if (out->max_arrv_rate) memcpy(out->max_arrv_rate, H(v.max_arrv_rate), S * 4);
+  Ext n;
+  n.S = S;
+  each_sol(n, [&](size_t c, int, auto* d, auto* o) { if (o) memcpy(o, H(d), c * sizeof(*d)); }, ctx->sol, *out);
   if (out->type_count) memcpy(out->type_count, H(ctx->d_type_count), T * 8);
   if (out->type_cost) memcpy(out->type_cost, H(ctx->d_type_cost), T * 8);
   return WVA_OK;

@@ -17,18 +17,18 @@ namespace wva {
 struct SatV2In {
   long long n_models, n_variants, n_replicas;
   const int *model_variant_off, *variant_replica_off;
-  const long long *rep_total_kv, *rep_tokens_in_use, *rep_queue_len, *rep_k2;
-  const double *rep_avg_in, *rep_avg_out, *rep_hit;
+  const long long *rep_total_kv_tokens, *rep_tokens_in_use, *rep_queue_length, *rep_k2;
+  const double *rep_avg_input_tokens, *rep_avg_output_tokens, *rep_prefix_hit_rate;
   const int* rep_slice_order;
   const int *var_current, *var_pending;
-  const double* var_fallback;
-  const double *cfg_kv_threshold, *cfg_scale_up, *cfg_scale_down;
-  const long long *sched_size, *sched_bytes;
+  const double* var_fallback_capacity;
+  const double *cfg_kv_threshold, *cfg_scale_up_threshold, *cfg_scale_down_boundary;
+  const long long *sched_queue_size, *sched_queue_bytes;
 };
 struct SatV2Out {
   long long *rep_k1, *rep_effective, *rep_demand; unsigned char* rep_saturated;
-  int* var_ready; double *var_cap, *var_total_cap, *var_total_demand, *var_util;
-  double *mod_supply, *mod_demand, *mod_util, *mod_required, *mod_spare;
+  int* var_ready; double *var_per_replica_capacity, *var_total_capacity, *var_total_demand, *var_utilization;
+  double *mod_total_supply, *mod_total_demand, *mod_utilization, *mod_required_capacity, *mod_spare_capacity;
 };
 
 // float64 -> int64 as Go does on amd64 (CVTTSD2SQ): NaN / out of range -> 0x8000000000000000
@@ -46,8 +46,8 @@ __device__ __forceinline__ double shfl_d(unsigned mask, double v, int src) {
 struct V2Rep { long long cap, in_use, queue, k2; double avg_in; };
 __device__ __forceinline__ V2Rep v2_load(const SatV2In& in, int r) {
   V2Rep x;
-  x.cap = in.rep_total_kv[r]; x.in_use = in.rep_tokens_in_use[r]; x.queue = in.rep_queue_len[r]; x.k2 = in.rep_k2[r];
-  x.avg_in = in.rep_avg_in[r];
+  x.cap = in.rep_total_kv_tokens[r]; x.in_use = in.rep_tokens_in_use[r]; x.queue = in.rep_queue_length[r]; x.k2 = in.rep_k2[r];
+  x.avg_in = in.rep_avg_input_tokens[r];
   return x;
 }
 // effective capacity of a replica (0 when it has no capacity data); also its demand
@@ -62,7 +62,7 @@ __device__ __forceinline__ bool v2_eval(const V2Rep& x, double kv_thr, long long
   return true;
 }
 __device__ __forceinline__ bool v2_replica(const SatV2In& in, int r, double kv_thr, long long& k1, long long& eff, long long& demand) {
-  if (in.rep_total_kv[r] <= 0) { k1 = 0; eff = 0; demand = 0; return false; }          // the other streams are not read
+  if (in.rep_total_kv_tokens[r] <= 0) { k1 = 0; eff = 0; demand = 0; return false; }   // the other streams are not read
   return v2_eval(v2_load(in, r), kv_thr, k1, eff, demand);
 }
 
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(256, V2_MINB) saturation_v2_kernel(SatV2In in,
           }
           cap = (double)((n_data % 2 == 0) ? (m_lo + m_hi) / 2 : m_hi);
         } else {
-          cap = in.var_fallback[v];                                                    // :317-324 (resolved by the caller)
+          cap = in.var_fallback_capacity[v];                                           // :317-324 (resolved by the caller)
         }
         const int pending = in.var_pending[v];
         int ready = in.var_current[v] - pending;                                        // :300-303
@@ -235,17 +235,17 @@ __global__ void __launch_bounds__(256, V2_MINB) saturation_v2_kernel(SatV2In in,
         if (total_cap > 0) util = d_div(demand_sum, total_cap);
         anticipated = d_mul((double)(ready + pending), cap);                           // Analyze :93-94
         if (out.var_ready) out.var_ready[v] = ready;
-        if (out.var_cap) out.var_cap[v] = cap;
-        if (out.var_total_cap) out.var_total_cap[v] = total_cap;
+        if (out.var_per_replica_capacity) out.var_per_replica_capacity[v] = cap;
+        if (out.var_total_capacity) out.var_total_capacity[v] = total_cap;
         if (out.var_total_demand) out.var_total_demand[v] = demand_sum;
-        if (out.var_util) out.var_util[v] = util;
+        if (out.var_utilization) out.var_utilization[v] = util;
       }
       // model sums in VariantStates order (Analyze :88-96); an inactive slot adds +0.0
       ordered_sums3(buf, lane, total_cap, demand_sum, anticipated, total_supply, total_demand, total_anticipated);
     }
     // scheduler queue demand (estimateSchedulerQueueDemand :471-501), only for the models that have one
-    const long long qs = in.sched_size ? in.sched_size[m] : 0, qb = in.sched_bytes ? in.sched_bytes[m] : 0;
-    if (in.sched_size && !(qs == 0 && qb == 0)) {
+    const long long qs = in.sched_queue_size ? in.sched_queue_size[m] : 0, qb = in.sched_queue_bytes ? in.sched_queue_bytes[m] : 0;
+    if (in.sched_queue_size && !(qs == 0 && qb == 0)) {
       // computeModelWorkloadAverages (:438-455): float64 sums over the model's replicas in SLICE order; the lanes
       // fetch 32 replicas per round trip, the adds run in order through shuffles
       const int r0 = R0, r1 = R1;
@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(256, V2_MINB) saturation_v2_kernel(SatV2In in,
         bool use = false;
         if (pos < r1) {
           const int r = in.rep_slice_order ? in.rep_slice_order[pos] : pos;
-          xi = in.rep_avg_in[r]; xo = in.rep_avg_out[r]; xh = in.rep_hit[r];
+          xi = in.rep_avg_input_tokens[r]; xo = in.rep_avg_output_tokens[r]; xh = in.rep_prefix_hit_rate[r];
           use = xi > 0 || xo > 0;
         }
         const unsigned um = __ballot_sync(full, use);
@@ -277,16 +277,16 @@ __global__ void __launch_bounds__(256, V2_MINB) saturation_v2_kernel(SatV2In in,
       double utilization = 0.0;
       if (total_supply > 0) utilization = d_div(total_demand, total_supply);           // :101-104
       double required = 0.0, spare = 0.0;
-      const double up = in.cfg_scale_up[m], down = in.cfg_scale_down[m];
+      const double up = in.cfg_scale_up_threshold[m], down = in.cfg_scale_down_boundary[m];
       if (up > 0) required = d_sub(d_div(total_demand, up), total_anticipated);        // :108-113
       if (required < 0) required = 0.0;
       if (down > 0) spare = d_sub(total_supply, d_div(total_demand, down));            // :115-120
       if (spare < 0) spare = 0.0;
-      if (out.mod_supply) out.mod_supply[m] = total_supply;
-      if (out.mod_demand) out.mod_demand[m] = total_demand;
-      if (out.mod_util) out.mod_util[m] = utilization;
-      if (out.mod_required) out.mod_required[m] = required;
-      if (out.mod_spare) out.mod_spare[m] = spare;
+      if (out.mod_total_supply) out.mod_total_supply[m] = total_supply;
+      if (out.mod_total_demand) out.mod_total_demand[m] = total_demand;
+      if (out.mod_utilization) out.mod_utilization[m] = utilization;
+      if (out.mod_required_capacity) out.mod_required_capacity[m] = required;
+      if (out.mod_spare_capacity) out.mod_spare_capacity[m] = spare;
     }
   }
 }

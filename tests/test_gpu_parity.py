@@ -555,6 +555,31 @@ def test_saturation_matches_oracle(pkg, engine, oracle, M, V, stream):
     assert (o["mod_flags"] & 1).any() and (o["mod_flags"] & 4).any()
 
 
+def test_saturation_rejected_upload_keeps_previous_batch(pkg, engine, oracle):
+    """An upload rejected for a missing required array (a larger batch, rep_kv NULL) is rejected before anything is
+    reserved or copied: the batch uploaded before it stays resident and runs to the same results."""
+    import ctypes
+    a = pkg.synth.saturation_batch(20, 4, stream=46)
+    o = oracle.saturation_v1(a)
+
+    def check(g):
+        for k in ("var_target", "var_replica_count", "var_non_saturated", "var_max_queue", "rep_saturated",
+                  "mod_total_replicas", "mod_non_saturated", "mod_flags", "partials"):
+            assert np.array_equal(g[k], o[k]), k
+        for k in ("var_max_kv", "var_avg_spare_kv", "var_avg_spare_queue", "mod_avg_spare_kv", "mod_avg_spare_queue"):
+            assert _bit_equal(g[k], o[k]), k
+
+    engine.saturation_upload(a)
+    engine.saturation_run(detail=True)
+    check(engine.saturation_fetch(detail=True))
+    b = pkg.synth.saturation_batch(400, 32, stream=47)   # large enough that the arenas would have to grow
+    ist, keep = pkg._abi.make_saturation_in(b)
+    ist.rep_kv = None
+    assert engine.lib.wva_saturation_upload(engine.ctx, ctypes.byref(ist)) == pkg._abi.WVA_ERR_ARG
+    engine.saturation_run(detail=True)
+    check(engine.saturation_fetch(detail=True))
+
+
 def test_saturation_ragged(pkg, engine, oracle):
     """variants without replicas, variants without state, models without variants, empty batch."""
     d = pkg.synth.saturation_batch(40, 6, stream=44)
