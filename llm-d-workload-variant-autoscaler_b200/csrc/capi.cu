@@ -572,15 +572,12 @@ int32_t wva_calculate(wva_ctx* ctx) {
     const bool pool_auto = !ctx->force_lane_sizer && n_pairs > (unsigned long long)ctx->sm_count * 640 && nmax <= 4096;
     if (pool_auto || (ctx->force_lane_sizer && ctx->lane_sizer_mode == 6)) {
       const int P = POOL_PMAX;
-      const int row_stride = (nmax + 31) & ~31;
       const size_t pool_bytes = (size_t)ctx->sm_count * P * sizeof(PoolEntry);
-      const size_t rows_bytes = (size_t)ctx->sm_count * P * (size_t)row_stride * 4;
-      CK(ctx->pool_ws.reserve(pool_bytes + rows_bytes + 512));
+      CK(ctx->pool_ws.reserve(pool_bytes + 512));
       PoolEntry* pool = (PoolEntry*)ctx->pool_ws.p;
-      float* rows = (float*)((char*)ctx->pool_ws.p + ((pool_bytes + 255) & ~(size_t)255));
       CK(cudaFuncSetAttribute(sizer_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PoolSmem)));
-      sizer_pool_kernel<<<ctx->sm_count, POOL_THREADS, sizeof(PoolSmem), ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, P, pool, rows,
-                                                                                        row_stride, ctx->d_ctr, d_ovf);
+      sizer_pool_kernel<<<ctx->sm_count, POOL_THREADS, sizeof(PoolSmem), ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, P, pool,
+                                                                                        ctx->d_ctr, d_ovf);
       ctx->launches++;
       cudaError_t pe = cudaGetLastError();
       if (pe != cudaSuccess) { ctx->last_error = std::string("pool sizer launch: ") + cudaGetErrorString(pe); return WVA_ERR_CUDA; }

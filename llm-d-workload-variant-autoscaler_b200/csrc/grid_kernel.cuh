@@ -63,22 +63,21 @@ __device__ __forceinline__ bool grid_store(const GridOut& out, size_t o, const P
 // Deferral of the near-saturation levels (large systems).  A pair's chain length is a steep function of lambda / mu_N
 // (early exit E4): the one or two lowest admitted levels of a pair run thousands of states next to ~50 for the rest, so a
 // warp that takes 32 consecutive levels spends its first round waiting for one lane.  With deferral the pair's warp skips
-// the levels whose ratio exceeds `thr`, saves the pair's head table (one row) and model, and appends (pair, r, class)
-// to a global list; the list is radix-sorted by length class and grid_deferred_kernel solves it 32 items — of 32
-// different pairs, similar lengths — at a time through TileTable.  Same per-level arithmetic, same outputs.
+// the levels whose ratio exceeds `thr`, saves the pair's model (without its head table: m.tab == nullptr), and appends
+// (pair, r, class) to a global list; the list is radix-sorted by length class and grid_deferred_kernel solves it 32
+// items — of 32 different pairs, similar lengths — at a time, each lane computing its own pair's rates (RateTable).
+// Same per-level arithmetic, same outputs.
 struct GridSide {            // what an evaluation needs of its pair
   PairModel m;
   float total_rate, slo_ttft, slo_itl, slo_tps, lambda_tps;
   int pad_[3];
 };
 struct GridDefer {
-  float* rows;               // [n_pairs][row_stride] head tables, nullptr = no deferral
-  GridSide* side;            // [n_pairs]
+  GridSide* side;            // [n_pairs], nullptr = no deferral
   unsigned long long* items; // (pair << 16) | r
   unsigned char* cls;        // length class of the item (sort key)
   unsigned long long* n_items;
   unsigned long long cap;
-  int row_stride;
   float thr;
 };
 __device__ __forceinline__ int grid_class(const PairModel& m, float ratio) {
@@ -155,8 +154,8 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
     model_finish(m, tabf, 1);
     const float lambda_tps = f_mul(m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));
     int front = 0x7fffffff;
-    const bool deferring = df.rows != nullptr && pair < 0xffffffffull;
-    bool saved = false;                                   // the pair's row and model are written when its first level is deferred
+    const bool deferring = df.side != nullptr && pair < 0xffffffffull;
+    bool saved = false;                                   // the pair's model is written when its first level is deferred
     const float mu_last_f = (float)m.mu_last;
     bool first_round = true;
 
@@ -210,11 +209,9 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
             }
             if (room > 0 && !saved) {                       // warp-uniform: the first level of the pair that leaves
               saved = true;
-              float* row = df.rows + (size_t)pair * df.row_stride;
-              for (int n = lane; n < m.N; n += 32) row[n] = tabf[n];
               if (lane == 0) {
                 GridSide sd;
-                sd.m = m; sd.m.tab = row; sd.m.stride = 1;
+                sd.m = m; sd.m.tab = nullptr; sd.m.stride = 0;
                 sd.total_rate = total_rate; sd.slo_ttft = slo_ttft; sd.slo_itl = slo_itl; sd.slo_tps = slo_tps; sd.lambda_tps = lambda_tps;
                 df.side[pair] = sd;
               }
@@ -285,10 +282,8 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
 __global__ void __launch_bounds__(256, 2)
 grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long* __restrict__ items, unsigned long long n_items,
                      GridCounters* ctr, unsigned long long* next_item, GridOverflowList ol) {
-  extern __shared__ __align__(16) float grid_tiles[];
   const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned tile = (unsigned)__cvta_generic_to_shared(grid_tiles + (size_t)warp * TileTable::kWarpFloats);
+  const int lane = threadIdx.x & 31;
   unsigned long long my_solves = 0, my_states = 0, my_slots = 0, my_rounds = 0;
   while (true) {
     unsigned long long i0 = 0;
@@ -311,8 +306,7 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
     int sv = 0;
     bool bad = false, ovf = false;
     if (uniform) {
-      TileTable tt; tt.rows = df.rows; tt.row_stride = df.row_stride; tt.slot = (int)pair; tt.tile = tile; tt.n_head = nref - 1;
-      sv = lockstep_solve_fast(m, tt, lambda, live, st, &ctr->certify_fallbacks);
+      sv = lockstep_solve_fast(m, RateTable{rate_coef(m)}, lambda, live, st, &ctr->certify_fallbacks);
       bad = sv < 0;
       if (bad) sv = -1 - sv;
     } else if (live) {

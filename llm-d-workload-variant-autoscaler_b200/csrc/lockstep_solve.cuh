@@ -50,83 +50,30 @@ struct LaneTable {   // one float32 column per lane ([n][thread], bank = lane); 
   __device__ __forceinline__ double mu_at(int n) const { return (double)t[(size_t)n * stride]; }
   __device__ __forceinline__ void prepare(int) const {}
 };
-// Rows in global memory, one per pool slot, and any 32 of them solved together (sizer_pool_kernel.cuh): the warp keeps
-// two shared tiles of 32 head states x 32 lanes.  Tile k+1 is fetched with cp.async (no registers, no scoreboard) while
-// the lanes work on tile k, so the only exposed latency is the first tile of a pass.  A tile is lane-major: lane l's 32
-// states are 8 chunks of 4 states (16 bytes) at l * 128 bytes, chunk c stored in place c ^ (l & 7), so that the
-// 16-byte reads of 8 consecutive lanes hit 8 different bank quads (conflict-free) and a chunk of 16 states is 4 loads.
-// The fetch moves 4 rows per cp.async instruction (8 lanes x 16 bytes per row: coalesced 128-byte accesses), 8
-// instructions and 8 shuffles of the row index per tile.  The tile is held as a shared-space address and read with
-// ld.shared (a generic pointer would be read with generic loads), and the table is passed by value, so that a
-// __noinline__ solver keeps its fields in registers.  Only (E1) rows are read through it (the pool queues and the
-// deferred grid pass take no other pair), so the loads convert on the integer pipe (f32pos_to_d, rcp_f32den_e1).
-struct TileTable {
+// Each lane's own rates, computed where they are used (sizer_pool_kernel.cuh, grid_deferred_kernel): any 32 pairs solve
+// together with no table in memory.  Entry n is serv_rate(n + 1) — the function BuildModel's table is filled with, so
+// the same bits — from the model's coefficients, held by value so that a __noinline__ solver keeps them in registers.
+// The float32 batch size is counted up by 1.0f (exact below 2^24).  A chunk's CH rates are formed before the
+// recurrence that uses them and do not depend on it: their float32 divisions run on the FP32 pipe, which the
+// FP64-bound head pass leaves idle.  Only (E1) models are solved through it (the pool queues and the deferred grid pass
+// take no other pair), so the conversions run on the integer pipe (f32pos_to_d, rcp_f32den_e1).
+struct RateTable {
   static constexpr int kChunk = WVA_TILE_CHUNK;   // states per unrolled chunk of the solver (code size vs loop overhead)
-  static constexpr int kWarpFloats = 2 * 32 * 32; // shared floats per warp (two tiles)
-  static_assert(32 % kChunk == 0 && kChunk % 4 == 0, "a chunk lies inside one tile and is whole 16-byte groups");
-  const float* rows;      // base of the CTA's rows (16-byte aligned)
-  int row_stride;         // floats per row (a multiple of 32, >= N)
-  int slot;               // this lane's row (any valid row for an idle lane)
-  unsigned tile;          // shared-space address of the warp's two tiles (kWarpFloats, 16-byte aligned)
-  int n_head;             // head entries (N - 1): tiles beyond are never fetched
-  // shared address of the 16 bytes of lane l's row holding states n .. n+3 (n a multiple of 4)
-  __device__ __forceinline__ unsigned group_addr(unsigned l, int n) const {
-    return tile + (((unsigned)n >> 5) & 1u) * 4096u + l * 128u + (((((unsigned)n >> 2) & 7u) ^ (l & 7u)) << 4);
-  }
-  __device__ __forceinline__ void fetch(int n0) const {
-    const unsigned lane = threadIdx.x & 31, c = lane & 7;
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      const unsigned l = 4 * k + (lane >> 3);      // the row (lane) this lane copies 16 bytes of
-      const int sr = __shfl_sync(0xffffffffu, slot, l);
-      const float* src = rows + (size_t)sr * row_stride + n0 + 4 * c;
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(group_addr(l, n0 + 4 * c)), "l"(src) : "memory");
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  }
-  // shared address of this lane's entry of state n
-  __device__ __forceinline__ unsigned addr(int n) const { return group_addr(threadIdx.x & 31, n & ~3) + 4u * (n & 3); }
-  // volatile: kept after the cp.async wait and __syncwarp of prepare()
-  static __device__ __forceinline__ float lds(unsigned a) {
-    float v;
-    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
-    return v;
-  }
-  static __device__ __forceinline__ float4 lds4(unsigned a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
-    return v;
-  }
-  __device__ __forceinline__ void prepare(int n) const {
-    if (n & 31) return;
-    if (n == 0) {                                               // first tile of a pass
-      asm volatile("cp.async.wait_group 0;" ::: "memory");      // a tile still in flight from a pass that ended early
-      __syncwarp();
-      fetch(0);
-    }
-    if (n + 32 < n_head) {                                      // next tile in flight while this one is used
-      __syncwarp();                                             // (its buffer was last read two tiles ago)
-      fetch(n + 32);
-      asm volatile("cp.async.wait_group 1;" ::: "memory");
-    } else {
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-    }
-    __syncwarp();
-  }
+  RateCoef c;
+  // a lane with no pair: mu_n = n + 1, every entry an (E1) divisor
+  static __device__ __forceinline__ RateTable idle() { return RateTable{{1.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f}}; }
+  __device__ __forceinline__ void prepare(int) const {}
   __device__ __forceinline__ void load(int n, double& mu, double& r) const {
-    float m32 = lds(addr(n)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
+    const float m32 = serv_rate_nf(c, (float)(n + 1)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
   }
   template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
-    const unsigned l = threadIdx.x & 31;
+    float m32[CH], nf = (float)(n + 1);
 #pragma unroll
-    for (int g = 0; g < CH / 4; g++) {
-      const float4 v = lds4(group_addr(l, n + 4 * g));
-      const float m32[4] = {v.x, v.y, v.z, v.w};
+    for (int j = 0; j < CH; j++) { m32[j] = serv_rate_nf(c, nf); nf = f_add(nf, 1.0f); }
 #pragma unroll
-      for (int e = 0; e < 4; e++) { mu[4 * g + e] = f32pos_to_d(m32[e]); r[4 * g + e] = rcp_f32den_e1(m32[e], mu[4 * g + e]); }
-    }
+    for (int j = 0; j < CH; j++) { mu[j] = f32pos_to_d(m32[j]); r[j] = rcp_f32den_e1(m32[j], mu[j]); }
   }
-  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(lds(addr(n))); }
+  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(serv_rate_nf(c, (float)(n + 1))); }
 };
 
 // high word of v * 2^-54 for a normal v >= 2^-900: the exponent field moves, nothing rounds
@@ -530,7 +477,7 @@ __device__ __forceinline__ void fast_chunk(FastHead& h, double lam, const double
 }
 
 // Phase profile of the fast solve (tools/perf_pool_phases.py): built with -DWVA_POOL_PHASES, lockstep_solve_fast_only
-// adds lane 0's clock64() cycles of the first tile wait, the head chunks (the later tile waits included) and
+// adds lane 0's clock64() cycles of the first chunk's table preparation (nothing for RateTable), the head chunks and
 // fast_solve_finish to ph[0..2].  The product build compiles none of it.
 #ifdef WVA_POOL_PHASES
 #define FAST_PH(...) __VA_ARGS__

@@ -4,8 +4,9 @@
 // longest of 32 chains that happen to sit in one warp: 49 % of the executed lane-steps do live work on BASELINE
 // configs[2] (59-62 % with the probe-sorted queue).  Chain length is almost a function of lambda / mu_N alone (early exit
 // E4), and it changes from one bisection step of a pair to the next — so here the binding is dropped:
-//   * a CTA keeps a pool of P pairs whose state (the SizerLane of wva_core.cuh) and head-table rows live in global
-//     memory (L2-resident: ~1.4 KB per pair at N = 256);
+//   * a CTA keeps a pool of P pairs whose state (the SizerLane of wva_core.cuh) lives in global memory (L2-resident:
+//     368 bytes per pair); a pair has no head table (m.tab == nullptr): its service rates are computed where a solve
+//     needs them (RateTable, model_rate);
 //   * every solve a pair still needs is a REQUEST — the pair's slot — queued in shared memory by class: 28 fast classes
 //     keyed by the head length N (the cost of the certified fast solve, E12) and 4 exact classes keyed by the exact
 //     solver's chain-length estimate, which hold the solves the fast solve did not certify;
@@ -15,14 +16,14 @@
 //     not certify re-queues its pair into an exact class at the same rate; every other lane advances its pair's
 //     bisection / Size / Analyze state machine (sizer_on_solve, the same code as every other sizer), stores the state
 //     back and queues the pair's next request — or retires the pair and frees its slot.
-//   * Free slots are refilled with new pairs from the global work counter: setup runs lane by lane, then the warp builds
-//     the head rows of the lanes that need one together, 32 entries at a time.
+//   * Free slots are refilled with new pairs from the global work counter: setup runs lane by lane, then the warp scans
+//     the service rates of the lanes that need a model together, 32 entries at a time.
 // Which lanes solve which pairs together changes nothing in any pair's arithmetic: same solves, same order per pair,
 // same state machine — candidates are bit-identical to the lane sizer's (and the oracle's).  tools/proto/lockstep_sim.py
 // and the measured counters (WVA_SIZER_DEBUG) give 88-92 % live lane-steps.
 //
-// Head tables: one row per slot in global memory; 32 arbitrary rows are read through TileTable (lockstep_solve.cuh): the
-// warp stages 32 states of its 32 rows per step, each row a coalesced 128-byte load.
+// Head rates: each lane of a batch computes its own pair's rates from the model's coefficients (RateTable,
+// lockstep_solve.cuh) on the FP32 pipe, which the FP64-bound solvers leave idle; nothing is read per state.
 #pragma once
 #include "wva_core.cuh"
 #include "sizer_kernel.cuh"
@@ -43,9 +44,7 @@ struct PoolSmem {
   unsigned short free_list[POOL_PMAX];
   int head[POOL_NCLS], tail[POOL_NCLS];
   int n_free, in_pool, exhausted, lock;
-  float tiles[POOL_THREADS / 32][TileTable::kWarpFloats];
 };
-static_assert(offsetof(PoolSmem, tiles) % 16 == 0, "TileTable's tiles take 16-byte cp.async copies and loads");
 
 __device__ __forceinline__ void pool_lock(int* lock) {
   if ((threadIdx.x & 31) == 0) {
@@ -122,7 +121,7 @@ enum {
   PH_FAST_PARTIAL, PH_EXACT_PARTIAL,                              // batches of fewer than 32 requests
   PH_ROWS, PH_ITERS,
   PH_MODEL,                                                       // cycles of fast batches: model load (pool_load_model),
-  PH_FAST_WAIT0, PH_FAST_CHUNKS, PH_FAST_FINISH,                  // first tile wait, head chunks, fast_solve_finish
+  PH_FAST_WAIT0, PH_FAST_CHUNKS, PH_FAST_FINISH,                  // first table preparation, head chunks, fast_solve_finish
   PH_N
 };
 __device__ unsigned long long g_pool_phase[PH_N];
@@ -155,21 +154,20 @@ __device__ __noinline__ bool pool_pair_on_chain(PoolEntry& ze, const SysView& s,
 }
 
 __global__ void __launch_bounds__(POOL_THREADS, 1)
-sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, int P, PoolEntry* pool_all, float* rows_all,
-                  int row_stride, SizerCounters* ctr, int* overflow_list) {
+sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, int P, PoolEntry* pool_all,
+                  SizerCounters* ctr, int* overflow_list) {
   extern __shared__ __align__(16) unsigned char pool_smem_raw[];
   PoolSmem& sm = *reinterpret_cast<PoolSmem*>(pool_smem_raw);
   const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
 #ifdef WVA_POOL_PHASES
+  const int warp = threadIdx.x >> 5;
   __shared__ unsigned long long ph_acc[POOL_THREADS / 32][PH_N];
   for (int k = lane; k < PH_N; k += 32) ph_acc[warp][k] = 0;
   const long long ph_start = clock64();
 #endif
   const unsigned lt = (1u << lane) - 1u;
   PoolEntry* pool = pool_all + (size_t)blockIdx.x * P;
-  float* rows = rows_all + (size_t)blockIdx.x * P * row_stride;
-  const unsigned tile = (unsigned)__cvta_generic_to_shared(sm.tiles[warp]);
 
   for (int i = threadIdx.x; i < P; i += POOL_THREADS) sm.free_list[i] = (unsigned short)(P - 1 - i);
   if (threadIdx.x < POOL_NCLS) { sm.head[threadIdx.x] = 0; sm.tail[threadIdx.x] = 0; }
@@ -263,8 +261,8 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
     pushA = pushB = freeA = freeB = -1;
     if (finished) break;
 
-    // ---- new pairs into the reserved slots: setup lane by lane (nil and zero-load pairs need no table), then
-    //      BuildModel (queueanalyzer.go:95-124) with the whole warp, one row after the other
+    // ---- new pairs into the reserved slots: setup lane by lane (nil and zero-load pairs need no model), then
+    //      BuildModel (queueanalyzer.go:95-124) with the whole warp, one pair's rates after the other
     if (__any_sync(full, new_slot >= 0)) {
       POOL_PH(const unsigned ph_new = __ballot_sync(full, new_slot >= 0); POOL_PH_ADD(PH_ROWS, __popc(ph_new));)
       PoolEntry ze;
@@ -281,10 +279,12 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
           if (rc == SETUP_NEEDS_TABLE) { need_table = true; break; }
         }
       }
-      // each row: lane l computes entries l, l + 32, ...; the rate range needs its first and last entry, and the
-      // monotone region the LAST descent !(row[n-1] <= row[n]) (where model_finish's scan from the top stops): a max over n
+      // each pair's rates: lane l computes entries l, l + 32, ... and keeps none of them; the rate range needs the first
+      // and last entry, the monotone region the LAST descent !(row[n-1] <= row[n]) (where model_finish's scan from the
+      // top stops): a max over n, and e1_ok whether every entry is an (E1) divisor: an and over n (model_finish checks
+      // the entries below mono and the two ends of the non-decreasing rest, which bound every entry between them)
       float r0 = 0.0f, rl = 0.0f;
-      int mono = 0;
+      int mono = 0, e1_ok = 0;
       unsigned need = __ballot_sync(full, need_table);
       while (need) {
         const int src = __ffs(need) - 1;
@@ -298,12 +298,12 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
         b.pre_c = __shfl_sync(full, z.m.pre_c, src);
         b.dec_c = __shfl_sync(full, z.m.dec_c, src);
         b.N = __shfl_sync(full, z.m.N, src);
-        float* row = rows + (size_t)__shfl_sync(full, new_slot, src) * row_stride;
         float cur = 0.0f, carry = 0.0f, first = 0.0f;
         int desc = 0;
+        bool e1 = true;
         for (int n0 = 0; n0 < b.N; n0 += 32) {
           const int n = n0 + lane;
-          if (n < b.N) { cur = serv_rate(b, n + 1); __stcg(row + n, cur); }
+          if (n < b.N) { cur = serv_rate(b, n + 1); e1 = e1 && e1_divisor(cur); }
           float prev = __shfl_up_sync(full, cur, 1);
           if (lane == 0) prev = carry;
           if (n > 0 && n < b.N && !(prev <= cur)) desc = n;
@@ -312,20 +312,16 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
         }
         const float last = __shfl_sync(full, cur, (b.N - 1) & 31);
         desc = __reduce_max_sync(full, desc);
-        if (lane == src) { r0 = first; rl = last; mono = desc; }
+        const bool all_e1 = __all_sync(full, e1);
+        if (lane == src) { r0 = first; rl = last; mono = desc; e1_ok = all_e1; }
       }
       bool live = false;
-      __syncwarp();                                    // the rows' entries, written by every lane, are read back below
       if (need_table) {
         PairModel& m = z.m;
-        m.tab = rows + (size_t)new_slot * row_stride; m.stride = 1;
+        m.tab = nullptr; m.stride = 0;
         model_set_range(m, r0, rl);
         m.mono = mono;
-        // every entry an (E1) divisor?  The row is non-decreasing from mono on, so its ends bound it there; read through
-        // L2, where the lanes wrote it (L1 may still hold the slot's previous row)
-        int e1 = e1_divisor(__ldcg(m.tab + mono)) && e1_divisor(rl);
-        for (int n = 0; n < mono; n++) e1 &= (int)e1_divisor(__ldcg(m.tab + n));
-        m.e1_ok = e1;
+        m.e1_ok = e1_ok;
         m.mu_last = (double)rl;
         m.r_last = rcp_f32den(rl, m.mu_last);
         live = sizer_begin(z, s, out);
@@ -357,7 +353,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
     SolveStats st;
     if (uniform) {
       if (!live) { pm.m.N = nref; pm.m.K = nref + nref * WVA_QUEUE_TO_BATCH; pm.m.mono = 0; pm.m.mu_last = 1.0; pm.m.r_last = 1.0; }
-      TileTable tt; tt.rows = rows; tt.row_stride = row_stride; tt.slot = live ? my_slot : 0; tt.tile = tile; tt.n_head = nref - 1;
+      const RateTable tt = live ? RateTable{rate_coef(pm.m)} : RateTable::idle();
       if (exact) {
         lockstep_solve(pm.m, tt, x, live, st, sv, bad);
       } else {

@@ -170,7 +170,7 @@ struct PairModel {
   float lambda_min, lambda_max;  // Size(): RateRange.Min/1000, RateRange.Max/1000
   float rate_max;                // RateRange.Max (req/s)
   int e1_ok;                     // every mu_n is an (E1) divisor; else the pair is solved by the per-lane chain (chain_step)
-  // head table: mu_n as float32 at tab[n*stride], n in [0,N)
+  // head table: mu_n as float32 at tab[n*stride], n in [0,N); nullptr: mu_n = serv_rate(n + 1) (model_rate)
   const float* tab;
   int stride;
   int mono;         // mu is non-decreasing on [mono, N-1]
@@ -199,13 +199,20 @@ WVA_HD float prefill_time(const PairModel& m, float n) {
 WVA_HD float decode_time(const PairModel& m, float n) {
   return f_add(f_add(iteration_time(m, n), m.beta), m.dec_c);
 }
-// queueanalyzer.go:100-104: servRate[n-1] for batch size n
-WVA_HD float serv_rate(const PairModel& m, int n) {
-  float nf = (float)n;
-  float pre = prefill_time(m, nf);
-  float dec = f_mul(m.out_tok, decode_time(m, nf));
+// What the service rate of a batch size needs of its model (RateTable in lockstep_solve.cuh holds it in registers)
+struct RateCoef { float alpha, slope, beta, pre_c, dec_c, in_tok, out_tok; };
+WVA_HD RateCoef rate_coef(const PairModel& m) { return {m.alpha, m.slope, m.beta, m.pre_c, m.dec_c, m.in_tok, m.out_tok}; }
+// queueanalyzer.go:100-104: servRate[n-1] for the float32 batch size nf = n (prefill_time, decode_time spelled out)
+WVA_HD float serv_rate_nf(const RateCoef& c, float nf) {
+  const float it = f_add(c.alpha, f_mul(nf, c.slope));
+  const float pre = c.in_tok == 0.0f ? 0.0f : f_add(it, c.pre_c);
+  const float dec = f_mul(c.out_tok, f_add(f_add(it, c.beta), c.dec_c));
   return f_div(nf, f_add(pre, dec));
 }
+WVA_HD float serv_rate(const PairModel& m, int n) { return serv_rate_nf(rate_coef(m), (float)n); }
+// mu_n (n in [0, N)) of a model: its head table, or serv_rate itself for a model without one (m.tab == nullptr: the pool
+// sizer and the deferred grid pass compute their rates instead of storing them)
+WVA_HD float model_rate(const PairModel& m, int n) { return m.tab ? m.tab[(size_t)n * m.stride] : serv_rate(m, n + 1); }
 
 // BuildModel (queueanalyzer.go:95-124): fills the head table for entries
 // [first, N) step `step` (so a warp can fill one table cooperatively).
@@ -283,7 +290,7 @@ WVA_HD double chain_next(const Chain& c, const PairModel& m, bool* exit_ok) {
   double mu, r;
   bool mono_ok;
   if (c.n < m.N - 1) {
-    float m32 = m.tab[(size_t)c.n * m.stride];
+    float m32 = model_rate(m, c.n);
     mu = (double)m32;
     r = rcp_f32den(m32, mu);
     mono_ok = (c.n >= m.mono) && (d_bits(c.lamg) <= d_bits(mu));
@@ -367,7 +374,7 @@ WVA_HD void literal_solve(const PairModel& m, float lambda, double* p, SolveStat
   const double scale = DBL_MAX / (double)K;
   double sRate = 0.0;
   for (int n = 0; n < K; n++) {
-    sRate = (double)m.tab[(size_t)(n < num ? n : num - 1) * m.stride];
+    sRate = (double)model_rate(m, n < num ? n : num - 1);
     p[n + 1] = d_div(d_mul(p[n], lam), sRate);
     int guard = 0;
     while (p[n + 1] < 0.0 || p[n + 1] > DBL_MAX || p[n + 1] != p[n + 1]) {
@@ -549,7 +556,7 @@ WVA_HD bool fast_solve_finish(const PairModel& m, float lambda, const FastHead& 
 }
 
 // One fast solve on a single lane (the host replay of lockstep_solve_fast; the device runs the same steps, chunks
-// and exit tests with the table prefetched into shared memory).  Returns whether it is certified.
+// and exit tests with each lane's rates in registers).  Returns whether it is certified.
 WVA_HD bool fast_solve(const PairModel& m, float lambda, SolveStats& st, int* states) {
   *states = 0;
   if (!m.e1_ok) return false;   // the device never gives such a pair to the fast solve
@@ -560,9 +567,9 @@ WVA_HD bool fast_solve(const PairModel& m, float lambda, SolveStats& st, int* st
   int n = 0;
   while (n < NH) {
     const int cnt = NH - n < WVA_TILE_CHUNK ? NH - n : WVA_TILE_CHUNK;
-    const double mu0 = (double)m.tab[(size_t)n * m.stride];
+    const double mu0 = (double)model_rate(m, n);
     for (int j = 0; j < cnt; j++) {
-      const float m32 = m.tab[(size_t)(n + j) * m.stride];
+      const float m32 = model_rate(m, n + j);
       const double mu = (double)m32, r = rcp_f32den(m32, mu);
       const double x = d_mul(h.p, lam);
       if (!in_window(x)) h.ok = false;

@@ -8,13 +8,16 @@
 // batch), first tile wait included, as tools/perf_pool_phases.py counts them; with 16 and with 4 working warps per SM
 // (4 and 1 per scheduler: the pipe-bound and the latency-bound figure).
 //
-//   product  lockstep_solve_fast_only itself (its head-pass counter, built with -DWVA_POOL_PHASES)
+//   product  lockstep_solve_fast_only itself over the rows (its head-pass counter, built with -DWVA_POOL_PHASES)
 //   base     the same head loop written out here: TileTable::load_chunk + fast_chunk + the chunk-boundary exit
+//   computed the same head loop over RateTable (lockstep_solve.cuh): each lane computes its rates from its model's
+//            coefficients, no row is read (what the pool sizer and the deferred grid pass run)
 //   (a) reg  the tile read replaced by values in registers: no ld.shared, conversion, rcp seed, refinement or λ·r per state
 //   (b) nof  the tile fetch hoisted out: both tiles fetched once at the start of a pass, no shfl / cp.async after it
 //   (d) noTA fast_chunk without the T / A accumulations (p1_chunk: the recurrence and the sum only)
 //   (c) CH = 8 is the same program built with -DWVA_TILE_CHUNK=8 (head_chunk_ch8).
-// The variants are measurements only: (a) and (b) read wrong table values and (d) drops what certification needs.
+// The variants (a), (b), (d) are measurements only: (a) and (b) read wrong table values and (d) drops what
+// certification needs.  TileTable, which streamed the pool's rows before RateTable replaced them, is kept here.
 //
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --fmad=false -DWVA_POOL_PHASES \
 //          -I../../llm-d-workload-variant-autoscaler_b200/csrc -o head_chunk head_chunk.cu        (add -DWVA_TILE_CHUNK=8 for (c))
@@ -30,22 +33,98 @@ using namespace wva;
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e_)); exit(1); } } while (0)
 
 constexpr int THREADS = 512, P = 1024, N = 256, STRIDE = 256;
-enum { V_PRODUCT, V_BASE, V_REG, V_NOFETCH, V_NOTA, V_COUNT };
-static const char* kNames[V_COUNT] = {"product", "base", "(a) reg", "(b) nof", "(d) noTA"};
+enum { V_PRODUCT, V_BASE, V_COMPUTED, V_REG, V_NOFETCH, V_NOTA, V_COUNT };
+static const char* kNames[V_COUNT] = {"product", "base", "computed", "(a) reg", "(b) nof", "(d) noTA"};
+
+// Rows in global memory, one per pool slot, and any 32 of them solved together: the warp keeps two shared tiles of 32
+// head states x 32 lanes.  Tile k+1 is fetched with cp.async while the lanes work on tile k, so the only exposed
+// latency is the first tile of a pass.  A tile is lane-major: lane l's 32 states are 8 chunks of 4 states (16 bytes) at
+// l * 128 bytes, chunk c stored in place c ^ (l & 7) (conflict-free 16-byte reads); a chunk of 16 states is 4 loads.
+struct TileTable {
+  static constexpr int kChunk = WVA_TILE_CHUNK;
+  static constexpr int kWarpFloats = 2 * 32 * 32; // shared floats per warp (two tiles)
+  static_assert(32 % kChunk == 0 && kChunk % 4 == 0, "a chunk lies inside one tile and is whole 16-byte groups");
+  const float* rows;      // base of the CTA's rows (16-byte aligned)
+  int row_stride;         // floats per row (a multiple of 32, >= N)
+  int slot;               // this lane's row
+  unsigned tile;          // shared-space address of the warp's two tiles (kWarpFloats, 16-byte aligned)
+  int n_head;             // head entries (N - 1): tiles beyond are never fetched
+  __device__ __forceinline__ unsigned group_addr(unsigned l, int n) const {
+    return tile + (((unsigned)n >> 5) & 1u) * 4096u + l * 128u + (((((unsigned)n >> 2) & 7u) ^ (l & 7u)) << 4);
+  }
+  __device__ __forceinline__ void fetch(int n0) const {
+    const unsigned lane = threadIdx.x & 31, c = lane & 7;
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+      const unsigned l = 4 * k + (lane >> 3);
+      const int sr = __shfl_sync(0xffffffffu, slot, l);
+      const float* src = rows + (size_t)sr * row_stride + n0 + 4 * c;
+      asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(group_addr(l, n0 + 4 * c)), "l"(src) : "memory");
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  }
+  __device__ __forceinline__ unsigned addr(int n) const { return group_addr(threadIdx.x & 31, n & ~3) + 4u * (n & 3); }
+  static __device__ __forceinline__ float lds(unsigned a) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
+    return v;
+  }
+  static __device__ __forceinline__ float4 lds4(unsigned a) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+    return v;
+  }
+  __device__ __forceinline__ void prepare(int n) const {
+    if (n & 31) return;
+    if (n == 0) {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+      __syncwarp();
+      fetch(0);
+    }
+    if (n + 32 < n_head) {
+      __syncwarp();
+      fetch(n + 32);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncwarp();
+  }
+  __device__ __forceinline__ void load(int n, double& mu, double& r) const {
+    float m32 = lds(addr(n)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
+  }
+  template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
+    const unsigned l = threadIdx.x & 31;
+#pragma unroll
+    for (int g = 0; g < CH / 4; g++) {
+      const float4 v = lds4(group_addr(l, n + 4 * g));
+      const float m32[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 4; e++) { mu[4 * g + e] = f32pos_to_d(m32[e]); r[4 * g + e] = rcp_f32den_e1(m32[e], mu[4 * g + e]); }
+    }
+  }
+  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(lds(addr(n))); }
+};
 
 __device__ __forceinline__ unsigned hash32(unsigned x) {
   x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
   return x;
 }
 
-// one row per slot, BuildModel's service rates of a synthetic model; mono = the last descent
-__global__ void build_rows(float* rows, int* mono, int n_rows) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_rows) return;
+// the synthetic model of row i
+__device__ __forceinline__ PairModel row_model(int i) {
   const unsigned h = hash32(i * 2654435761u + 7u);
   PairModel m;
   model_init(m, 4.0f + (float)(h & 1023) * (8.0f / 1024.0f), 0.02f + (float)((h >> 10) & 255) * 1e-4f, 5e-4f,
              256 + (int)((h >> 18) & 1023), 64 + (int)((h >> 24) & 255), N);
+  return m;
+}
+
+// one row per slot, BuildModel's service rates of a synthetic model; mono = the last descent
+__global__ void build_rows(float* rows, int* mono, int n_rows) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_rows) return;
+  const PairModel m = row_model(i);
   float* row = rows + (size_t)i * STRIDE;
   int desc = 0;
   float prev = 0.0f;
@@ -171,6 +250,7 @@ head_kernel(const float* rows_all, const int* mono_all, int batches, int warps_o
     } else {
       const long long t0 = clock64();
       if (V == V_BASE) sv = head_loop<true>(m, tt, lambda, true, &keep);
+      if (V == V_COMPUTED) sv = head_loop<true>(m, RateTable{rate_coef(row_model(blockIdx.x * P + slot))}, lambda, true, &keep);
       if (V == V_NOFETCH) { NoFetchTable nf; static_cast<TileTable&>(nf) = tt; sv = head_loop<true>(m, nf, lambda, true, &keep); }
       if (V == V_NOTA) sv = head_loop<false>(m, tt, lambda, true, &keep);
       if (V == V_REG) {
@@ -227,6 +307,7 @@ int main(int argc, char** argv) {
   for (int w : {16, 4}) {
     run<V_PRODUCT>(sms, w, batches, rows, mono, acc, sink);
     run<V_BASE>(sms, w, batches, rows, mono, acc, sink);
+    run<V_COMPUTED>(sms, w, batches, rows, mono, acc, sink);
     run<V_REG>(sms, w, batches, rows, mono, acc, sink);
     run<V_NOFETCH>(sms, w, batches, rows, mono, acc, sink);
     run<V_NOTA>(sms, w, batches, rows, mono, acc, sink);

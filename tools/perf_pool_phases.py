@@ -3,7 +3,7 @@
 Builds the library of a source tree (default: this one) with -DWVA_POOL_PHASES into its own directory, runs
 System.Calculate on the pool sizer and prints each phase's share of the warps' clock64() cycles, and the live
 lane-steps of fast and exact batches.  The fast batches are split further into the model load (pool_load_model), the
-first tile wait of each head pass, the head chunks (the later tile waits included) and fast_solve_finish, and the head
+first table preparation of each head pass (a shared-memory tile wait when the rates were streamed from rows), the head chunks (the later tile waits included) and fast_solve_finish, and the head
 chunks' cycles are given per warp-state (one state index of a batch: 32 lane-steps, live or not) and per live lane-state.
 The product library in the tree is neither used nor touched.
 
@@ -27,7 +27,7 @@ NAMES = ["lock", "new_pairs", "fast", "exact", "state", "total", "fast_batches",
 PHASES = {"lock": "critical section", "new_pairs": "new-pair setup + BuildModel",
           "fast": "model load + fast head + finish", "exact": "exact solves",
           "state": "state load + sizer_on_solve + store"}
-FAST_PARTS = {"model": "model load", "fast_wait0": "first tile wait", "fast_chunks": "head chunks",
+FAST_PARTS = {"model": "model load", "fast_wait0": "first table preparation", "fast_chunks": "head chunks",
               "fast_finish": "fast_solve_finish"}
 
 
@@ -97,7 +97,7 @@ def main():
     res["chunk_cycles_per_live_lane_state"] = r["fast_chunks"] / max(r["fast_states"], 1)
     print(f"  head chunks: {res['chunk_cycles_per_warp_state']:.1f} cycles per warp-state "
           f"({warp_states:.3g} warp-states), {res['chunk_cycles_per_live_lane_state']:.2f} per live lane-state; "
-          f"first tile wait {r['fast_wait0'] / max(r['fast_batches'], 1):.0f} cycles per batch")
+          f"first table preparation {r['fast_wait0'] / max(r['fast_batches'], 1):.0f} cycles per batch")
     for kind in ("fast", "exact"):
         b, st, sl = r[f"{kind}_batches"], r[f"{kind}_states"], r[f"{kind}_slots"]
         print(f"  {kind} batches {b} ({r[kind + '_partial']} with < 32 requests): live lane-steps {st} of {sl} "
