@@ -55,25 +55,27 @@ struct LaneTable {   // one float32 column per lane ([n][thread], bank = lane); 
 // the same bits — from the model's coefficients, held by value so that a __noinline__ solver keeps them in registers.
 // The float32 batch size is counted up by 1.0f (exact below 2^24).  A chunk's CH rates are formed before the
 // recurrence that uses them and do not depend on it: their float32 divisions run on the FP32 pipe, which the
-// FP64-bound head pass leaves idle.  Only (E1) models are solved through it (the pool queues and the deferred grid pass
-// take no other pair), so the conversions run on the integer pipe (f32pos_to_d, rcp_f32den_e1).
+// FP64-bound head pass leaves idle.  Only models with e1_ok are solved through it (the pool queues and the deferred grid
+// pass take no other pair): every rate is an (E1) divisor, so the conversions run on the integer pipe (f32pos_to_d,
+// rcp_f32den_e1), and every denominator passed rate_den_ok, so the divisions are div_rate's branch-free sequence
+// (serv_rate_e1) and a chunk's rates are straight-line code the scheduler interleaves.
 struct RateTable {
   static constexpr int kChunk = WVA_TILE_CHUNK;   // states per unrolled chunk of the solver (code size vs loop overhead)
   RateCoef c;
-  // a lane with no pair: mu_n = n + 1, every entry an (E1) divisor
+  // a lane with no pair: mu_n = n + 1, every entry an (E1) divisor with den = 1
   static __device__ __forceinline__ RateTable idle() { return RateTable{{1.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f}}; }
   __device__ __forceinline__ void prepare(int) const {}
   __device__ __forceinline__ void load(int n, double& mu, double& r) const {
-    const float m32 = serv_rate_nf(c, (float)(n + 1)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
+    const float m32 = serv_rate_e1(c, (float)(n + 1)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
   }
   template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
     float m32[CH], nf = (float)(n + 1);
 #pragma unroll
-    for (int j = 0; j < CH; j++) { m32[j] = serv_rate_nf(c, nf); nf = f_add(nf, 1.0f); }
+    for (int j = 0; j < CH; j++) { m32[j] = serv_rate_e1(c, nf); nf = f_add(nf, 1.0f); }
 #pragma unroll
     for (int j = 0; j < CH; j++) { mu[j] = f32pos_to_d(m32[j]); r[j] = rcp_f32den_e1(m32[j], mu[j]); }
   }
-  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(serv_rate_nf(c, (float)(n + 1))); }
+  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(serv_rate_e1(c, (float)(n + 1))); }
 };
 
 // high word of v * 2^-54 for a normal v >= 2^-900: the exponent field moves, nothing rounds

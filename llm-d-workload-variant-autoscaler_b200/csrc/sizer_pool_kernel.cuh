@@ -312,7 +312,8 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
         }
         const float last = __shfl_sync(full, cur, (b.N - 1) & 31);
         desc = __reduce_max_sync(full, desc);
-        const bool all_e1 = __all_sync(full, e1);
+        // and the solves' RateTable may form the rates with div_rate: den(N) bounds every denominator
+        const bool all_e1 = __all_sync(full, e1) && rate_den_ok(rate_den(rate_coef(b), (float)b.N));
         if (lane == src) { r0 = first; rl = last; mono = desc; e1_ok = all_e1; }
       }
       bool live = false;

@@ -62,6 +62,7 @@ WVA_HD double d_add(double a, double b) { return __dadd_rn(a, b); }
 WVA_HD double d_sub(double a, double b) { return __dsub_rn(a, b); }
 WVA_HD double d_mul(double a, double b) { return __dmul_rn(a, b); }
 WVA_HD double d_div(double a, double b) { return __ddiv_rn(a, b); }
+WVA_HD float f_fma(float a, float b, float c) { return __fmaf_rn(a, b, c); }
 WVA_HD double d_fma(double a, double b, double c) { return __fma_rn(a, b, c); }
 WVA_HD double d_rcp(double a) { return __drcp_rn(a); }
 WVA_HD float f_rcp_approx(float a) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(a)); return r; }
@@ -76,6 +77,7 @@ WVA_HD double d_add(double a, double b) { return a + b; }
 WVA_HD double d_sub(double a, double b) { return a - b; }
 WVA_HD double d_mul(double a, double b) { return a * b; }
 WVA_HD double d_div(double a, double b) { return a / b; }
+WVA_HD float f_fma(float a, float b, float c) { return fmaf(a, b, c); }
 WVA_HD double d_fma(double a, double b, double c) { return fma(a, b, c); }
 WVA_HD double d_rcp(double a) { return 1.0 / a; }
 // rcp.approx.ftz: a subnormal input is read as 0 and a subnormal result is returned as 0
@@ -169,7 +171,8 @@ struct PairModel {
   int N, K;
   float lambda_min, lambda_max;  // Size(): RateRange.Min/1000, RateRange.Max/1000
   float rate_max;                // RateRange.Max (req/s)
-  int e1_ok;                     // every mu_n is an (E1) divisor; else the pair is solved by the per-lane chain (chain_step)
+  int e1_ok;                     // every mu_n is an (E1) divisor and den(N) passes rate_den_ok; else the pair is solved by
+                                 // the per-lane chain (chain_step)
   // head table: mu_n as float32 at tab[n*stride], n in [0,N); nullptr: mu_n = serv_rate(n + 1) (model_rate)
   const float* tab;
   int stride;
@@ -202,17 +205,54 @@ WVA_HD float decode_time(const PairModel& m, float n) {
 // What the service rate of a batch size needs of its model (RateTable in lockstep_solve.cuh holds it in registers)
 struct RateCoef { float alpha, slope, beta, pre_c, dec_c, in_tok, out_tok; };
 WVA_HD RateCoef rate_coef(const PairModel& m) { return {m.alpha, m.slope, m.beta, m.pre_c, m.dec_c, m.in_tok, m.out_tok}; }
-// queueanalyzer.go:100-104: servRate[n-1] for the float32 batch size nf = n (prefill_time, decode_time spelled out)
-WVA_HD float serv_rate_nf(const RateCoef& c, float nf) {
+// queueanalyzer.go:100-104: the denominator of servRate[n-1], PrefillTime + DecodeTime at the float32 batch size nf = n
+// (prefill_time, decode_time spelled out).  The coefficients are >= 0 (checked at load), so every operation is monotone
+// in nf: den(1) <= den(n) <= den(N) for n in [1, N].
+WVA_HD float rate_den(const RateCoef& c, float nf) {
   const float it = f_add(c.alpha, f_mul(nf, c.slope));
   const float pre = c.in_tok == 0.0f ? 0.0f : f_add(it, c.pre_c);
   const float dec = f_mul(c.out_tok, f_add(f_add(it, c.beta), c.dec_c));
-  return f_div(nf, f_add(pre, dec));
+  return f_add(pre, dec);
 }
+// servRate[n-1] (queueanalyzer.go:100-104) with the IEEE division
+WVA_HD float serv_rate_nf(const RateCoef& c, float nf) { return f_div(nf, rate_den(c, nf)); }
 WVA_HD float serv_rate(const PairModel& m, int n) { return serv_rate_nf(rate_coef(m), (float)n); }
+// RN(nf / den) without the IEEE division's range check and slow path, straight-line code: one Newton step on the seed s
+// gives y = RN(1/den), and Markstein's correction of q0 = RN(nf y) with the exact remainder gives the quotient.  Where
+// den's significand is all ones, 1/den = 2^k (1 + 2^-24 + ...) lies just above the midpoint between 2^k and
+// RN(1/den) = 2^k (1 + 2^-23), and from a seed below RN(1/den) the step rounds to 2^k (without the fix below the steps
+// are exact there only for a seed at RN(1/den)); setting the last bit maps both to RN(1/den).
+// It is the correctly rounded quotient when nf is an integer in [1, 2^16], den < 2^126 (rate_den_ok) and the quotient is
+// an (E1) divisor.  Then the seed is normal and within SEED_MAX_ULP of RN(1/den) (tests/test_device_prims.py), and s, y,
+// q0 and q are normal and finite (den >= 2^-126 follows from q <= 2^126), so the steps scale exactly with den's exponent;
+// tests/test_rate_division.py checks every den in [1, 2), every seed s that close and every nf.  Above 2^126 the seed
+// flushes to 0.
+WVA_HD float div_rate_seeded(float nf, float den, float s) {
+  const float r1 = f_fma(s, f_fma(-den, s, 1.0f), s);
+#if defined(__CUDA_ARCH__)
+  const unsigned db = __float_as_uint(den), rb = __float_as_uint(r1);
+  const float y = __uint_as_float(rb | (unsigned)(((db + 1u) & 0x7FFFFFu) == 0u));
+#else
+  unsigned db, rb; memcpy(&db, &den, 4); memcpy(&rb, &r1, 4);
+  rb |= (unsigned)(((db + 1u) & 0x7FFFFFu) == 0u);
+  float y; memcpy(&y, &rb, 4);
+#endif
+  const float q0 = f_mul(nf, y);
+  const float rem = f_fma(-den, q0, nf);
+  return f_fma(y, rem, q0);
+}
+WVA_HD float div_rate(float nf, float den) { return div_rate_seeded(nf, den, f_rcp_approx(den)); }
+// whether div_rate may divide by den(N), and so (rate_den is monotone) by every denominator of the pair
+WVA_HD bool rate_den_ok(float den) { return den < 0x1p126f; }
+// servRate[n-1] of an (E1) pair that passed rate_den_ok: the same bits as serv_rate_nf
+WVA_HD float serv_rate_e1(const RateCoef& c, float nf) { return div_rate(nf, rate_den(c, nf)); }
 // mu_n (n in [0, N)) of a model: its head table, or serv_rate itself for a model without one (m.tab == nullptr: the pool
 // sizer and the deferred grid pass compute their rates instead of storing them)
 WVA_HD float model_rate(const PairModel& m, int n) { return m.tab ? m.tab[(size_t)n * m.stride] : serv_rate(m, n + 1); }
+// model_rate of a pair with e1_ok, formed as RateTable forms it
+WVA_HD float model_rate_e1(const PairModel& m, int n) {
+  return m.tab ? m.tab[(size_t)n * m.stride] : serv_rate_e1(rate_coef(m), (float)(n + 1));
+}
 
 // BuildModel (queueanalyzer.go:95-124): fills the head table for entries
 // [first, N) step `step` (so a warp can fill one table cooperatively).
@@ -244,7 +284,8 @@ WVA_HD void model_finish(PairModel& m, const float* tab, int stride) {
   // mu is non-decreasing on [mono, N-1]: its ends bound it there, only the entries below mono are checked one by one
   int e1 = e1_divisor(tab[(size_t)mono * stride]) && e1_divisor(rl);
   for (int n = 0; n < mono; n++) e1 &= (int)e1_divisor(tab[(size_t)n * stride]);
-  m.e1_ok = e1;
+  // and the rates can be formed with div_rate (RateTable) where a solver computes them
+  m.e1_ok = e1 && rate_den_ok(rate_den(rate_coef(m), (float)m.N));
   m.mu_last = (double)rl;
   m.r_last = rcp_f32den(rl, m.mu_last);
 }
@@ -567,9 +608,9 @@ WVA_HD bool fast_solve(const PairModel& m, float lambda, SolveStats& st, int* st
   int n = 0;
   while (n < NH) {
     const int cnt = NH - n < WVA_TILE_CHUNK ? NH - n : WVA_TILE_CHUNK;
-    const double mu0 = (double)model_rate(m, n);
+    const double mu0 = (double)model_rate_e1(m, n);
     for (int j = 0; j < cnt; j++) {
-      const float m32 = model_rate(m, n + j);
+      const float m32 = model_rate_e1(m, n + j);
       const double mu = (double)m32, r = rcp_f32den(m32, mu);
       const double x = d_mul(h.p, lam);
       if (!in_window(x)) h.ok = false;

@@ -12,12 +12,14 @@
 //   base     the same head loop written out here: TileTable::load_chunk + fast_chunk + the chunk-boundary exit
 //   computed the same head loop over RateTable (lockstep_solve.cuh): each lane computes its rates from its model's
 //            coefficients, no row is read (what the pool sizer and the deferred grid pass run)
+//   ieee     computed with every rate divided by __fdiv_rn (IeeeRateTable, kept here): RateTable before div_rate
 //   (a) reg  the tile read replaced by values in registers: no ld.shared, conversion, rcp seed, refinement or λ·r per state
 //   (b) nof  the tile fetch hoisted out: both tiles fetched once at the start of a pass, no shfl / cp.async after it
 //   (d) noTA fast_chunk without the T / A accumulations (p1_chunk: the recurrence and the sum only)
 //   (c) CH = 8 is the same program built with -DWVA_TILE_CHUNK=8 (head_chunk_ch8).
 // The variants (a), (b), (d) are measurements only: (a) and (b) read wrong table values and (d) drops what
-// certification needs.  TileTable, which streamed the pool's rows before RateTable replaced them, is kept here.
+// certification needs.  TileTable, which streamed the pool's rows before RateTable replaced them, and IeeeRateTable,
+// RateTable before its divisions became div_rate, are kept here.
 //
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --fmad=false -DWVA_POOL_PHASES \
 //          -I../../llm-d-workload-variant-autoscaler_b200/csrc -o head_chunk head_chunk.cu        (add -DWVA_TILE_CHUNK=8 for (c))
@@ -33,8 +35,8 @@ using namespace wva;
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e_)); exit(1); } } while (0)
 
 constexpr int THREADS = 512, P = 1024, N = 256, STRIDE = 256;
-enum { V_PRODUCT, V_BASE, V_COMPUTED, V_REG, V_NOFETCH, V_NOTA, V_COUNT };
-static const char* kNames[V_COUNT] = {"product", "base", "computed", "(a) reg", "(b) nof", "(d) noTA"};
+enum { V_PRODUCT, V_BASE, V_COMPUTED, V_IEEE, V_REG, V_NOFETCH, V_NOTA, V_COUNT };
+static const char* kNames[V_COUNT] = {"product", "base", "computed", "ieee", "(a) reg", "(b) nof", "(d) noTA"};
 
 // Rows in global memory, one per pool slot, and any 32 of them solved together: the warp keeps two shared tiles of 32
 // head states x 32 lanes.  Tile k+1 is fetched with cp.async while the lanes work on tile k, so the only exposed
@@ -149,6 +151,22 @@ struct RegTable {             // (a): every state reads the same per-lane (mu, r
   __device__ __forceinline__ void load(int, double& m, double& rr) const { m = mu; rr = r; }
   __device__ __forceinline__ double mu_at(int) const { return mu; }
 };
+struct IeeeRateTable {        // ieee: RateTable with the IEEE division (serv_rate_nf), one slow-path branch per rate
+  static constexpr int kChunk = WVA_TILE_CHUNK;
+  RateCoef c;
+  __device__ __forceinline__ void prepare(int) const {}
+  __device__ __forceinline__ void load(int n, double& mu, double& r) const {
+    const float m32 = serv_rate_nf(c, (float)(n + 1)); mu = f32pos_to_d(m32); r = rcp_f32den_e1(m32, mu);
+  }
+  template <int CH> __device__ __forceinline__ void load_chunk(int n, double (&mu)[CH], double (&r)[CH]) const {
+    float m32[CH], nf = (float)(n + 1);
+#pragma unroll
+    for (int j = 0; j < CH; j++) { m32[j] = serv_rate_nf(c, nf); nf = f_add(nf, 1.0f); }
+#pragma unroll
+    for (int j = 0; j < CH; j++) { mu[j] = f32pos_to_d(m32[j]); r[j] = rcp_f32den_e1(m32[j], mu[j]); }
+  }
+  __device__ __forceinline__ double mu_at(int n) const { return f32pos_to_d(serv_rate_nf(c, (float)(n + 1))); }
+};
 struct NoFetchTable : TileTable {   // (b): tiles 0 and 1 fetched once per pass; later states read them again
   __device__ __forceinline__ void prepare(int n) const {
     if (n) return;
@@ -251,6 +269,7 @@ head_kernel(const float* rows_all, const int* mono_all, int batches, int warps_o
       const long long t0 = clock64();
       if (V == V_BASE) sv = head_loop<true>(m, tt, lambda, true, &keep);
       if (V == V_COMPUTED) sv = head_loop<true>(m, RateTable{rate_coef(row_model(blockIdx.x * P + slot))}, lambda, true, &keep);
+      if (V == V_IEEE) sv = head_loop<true>(m, IeeeRateTable{rate_coef(row_model(blockIdx.x * P + slot))}, lambda, true, &keep);
       if (V == V_NOFETCH) { NoFetchTable nf; static_cast<TileTable&>(nf) = tt; sv = head_loop<true>(m, nf, lambda, true, &keep); }
       if (V == V_NOTA) sv = head_loop<false>(m, tt, lambda, true, &keep);
       if (V == V_REG) {
@@ -308,6 +327,7 @@ int main(int argc, char** argv) {
     run<V_PRODUCT>(sms, w, batches, rows, mono, acc, sink);
     run<V_BASE>(sms, w, batches, rows, mono, acc, sink);
     run<V_COMPUTED>(sms, w, batches, rows, mono, acc, sink);
+    run<V_IEEE>(sms, w, batches, rows, mono, acc, sink);
     run<V_REG>(sms, w, batches, rows, mono, acc, sink);
     run<V_NOFETCH>(sms, w, batches, rows, mono, acc, sink);
     run<V_NOTA>(sms, w, batches, rows, mono, acc, sink);
