@@ -491,7 +491,8 @@ int32_t wva_limit(wva_ctx* ctx, int64_t n_decisions, int32_t n_types,
  * SaturationAnalyzer.Analyze (internal/engines/analyzers/saturation_v2/analyzer.go:59-138: computeReplicaCapacity
  * :142-211, aggregateByVariant :266-349, estimateSchedulerQueueDemand :471-501, median :505-519) for a batch of
  * models.  The arithmetic only: what the reference keeps in string-keyed state stays with the caller (SURVEY 8f.1) —
- * the k2 priority chain (computeK2 :218-262, rolling history) resolves rep_k2 per replica, the capacity store
+ * the k2 priority chain (computeK2 :218-262, rolling history) resolves rep_k2 per replica (on the device with
+ * wva_k2_resolve below), the capacity store
  * resolves var_fallback_capacity for variants without ready replicas (:317-324).
  * Variants of a model in VariantStates order; replicas of a variant in ReplicaMetrics order.
  */
@@ -570,6 +571,78 @@ int32_t wva_pipeline_v2(wva_ctx* ctx, const wva_saturation_v2_in* in, const doub
                         const uint8_t* mod_scale_to_zero_enabled, const double* mod_request_count,
                         const uint8_t* mod_request_error /* or NULL */, const wva_saturation_v2_out* out,
                         int32_t* var_target, uint8_t* mod_applied /* or NULL */);
+
+/* ---- V2 k2 priority chain with its rolling history in HBM -------------------- */
+/*
+ * SaturationAnalyzer.computeK2 (internal/engines/analyzers/saturation_v2/analyzer.go:218-262) for every replica of a
+ * cycle, with the analyzer's computeCapacityHistory (history.go, window RollingAverageWindowSize = 10, constants.go)
+ * kept on the device for the life of the handle.  What the reference does, and the device reproduces exactly:
+ *   - only replicas with TotalKvCapacityTokens > 0 run the chain (:148-150); the others neither read nor write history;
+ *     replicas of a variant without a VariantReplicaState still do (Analyze loops over every ReplicaMetrics, :73-84);
+ *   - the key is modelID|accelerator|bucket, without the namespace: the model groups (modelID|namespace,
+ *     internal/utils/variant.go:64-74) of one modelID share it.  A HISTORY GROUP here is one modelID; its model groups
+ *     are visited in registry order (one of Go's map orders), the replicas of a group in ReplicaMetrics slice order,
+ *     and an append is seen by every later replica of the same key in the same cycle;
+ *   - bucket (types.go:28-37): 0 short (avgOutput < 100), 1 medium (< 500), 2 long (otherwise, NaN included);
+ *   - priority 1, observed: queueLen >= int(QueueLengthThreshold) (Go amd64 conversion: NaN / out of range ->
+ *     INT64_MIN) && tokensInUse > 0: k2 = tokensInUse, appended to the key's window (the oldest value is dropped at 10);
+ *   - priority 2, historical: the window's float64 sum, oldest to newest, / float64(len); > 0: k2 = int64(avg);
+ *   - priority 3, derived: estimateCapacityFromParams (:418-437) with the VLLMParams of the store record
+ *     namespace|model|variant as of the start of the cycle (the per-replica Update keeps them, :184-196);
+ *   - priority 4: k2 = k1 = int64(float64(TotalKvCapacityTokens) * KvCacheThreshold); effective = min(k1, k2).
+ * The capacity store itself stays with the caller: FindCompatible (capacity_store.go:153-187) returns the first live
+ * record in map order, and the zero-replica fallback (:317-415) reads the store after this cycle's updates.  The
+ * resolve returns what the caller needs to apply those updates once per store slot (last write wins, :188-197).
+ * Nothing evicts keys (EvictStaleHistory has no caller in the reference); export / import is how a caller drops them.
+ *
+ * Registry (integers only; a change = export, create, import): H history groups; CSR history group -> model groups
+ * (every model group in [0, G) exactly once); CSR history group -> its distinct accelerator ids (the caller maps names,
+ * "" included, to ids >= 0); the number of store slots.  The keys of history group h are (accelerator k of h, bucket b)
+ * at index (hg_acc_off[h] + k) * 3 + b.
+ */
+typedef struct wva_k2_history wva_k2_history;
+int32_t wva_k2_history_create(wva_ctx* ctx, int64_t n_history_groups, int64_t n_model_groups, int64_t n_slots,
+                              const int32_t* hg_model_off /* [H+1] */, const int32_t* hg_models /* [G] */,
+                              const int32_t* hg_acc_off /* [H+1] */, const int32_t* hg_acc /* [hg_acc_off[H]] */,
+                              wva_k2_history** out);
+int32_t wva_k2_history_destroy(wva_k2_history* h);
+/* number of history keys: 3 * hg_acc_off[H] */
+int64_t wva_k2_history_keys(const wva_k2_history* h);
+
+typedef struct {
+  int64_t n_model_groups, n_replicas;       /* G must equal the registry's                                         */
+  const int32_t* model_replica_off;         /* [G+1] replicas of model group g in ReplicaMetrics slice order         */
+  const int64_t* rep_total_kv_tokens;       /* [P] TotalKvCapacityTokens; <= 0: no capacity data                      */
+  const int64_t* rep_tokens_in_use;         /* [P] */
+  const int64_t* rep_queue_length;          /* [P] */
+  const double* rep_avg_input_tokens;       /* [P] */
+  const double* rep_avg_output_tokens;      /* [P] */
+  const int32_t* rep_accelerator;           /* [P] accelerator id; must be registered for the group's history group   */
+  const int32_t* rep_slot;                  /* [P] store slot of namespace|model|variant, in [0, n_slots)             */
+  const int32_t* rep_out_pos;               /* [P] or NULL: position in a wva_saturation_v2_in layout, -1 = not there */
+  int64_t n_out;                            /* size of that layout (out_rep_k2)                                       */
+  const int64_t* slot_max_batched_tokens;   /* [S] VLLMParams.EffectiveMaxBatchedTokens (0 = no params)               */
+  const int64_t* slot_max_num_seqs;         /* [S] VLLMParams.MaxNumSeqs                                              */
+  const double* cfg_queue_threshold;        /* [G] SaturationScalingConfig.QueueLengthThreshold                       */
+  const double* cfg_kv_threshold;           /* [G] KvCacheThreshold                                                  */
+} wva_k2_in;
+typedef struct {
+  int64_t* rep_k2;          /* [P] computeK2's result; -1 without capacity data (wva_saturation_v2_in.rep_k2 as is)   */
+  int64_t* rep_effective;   /* [P] min(k1, k2); 0 without capacity data (may be NULL)                                  */
+  int64_t* out_rep_k2;      /* [n_out] rep_k2 scattered to rep_out_pos, -1 elsewhere (NULL unless rep_out_pos given)   */
+  int32_t* slot_last_rep;   /* [S] index of the slot's last data replica of the cycle, -1 = none (may be NULL)        */
+  int64_t* slot_effective;  /* [S] that replica's EffectiveCapacity, 0 = none (may be NULL)                           */
+} wva_k2_out;
+/* One cycle: appends to the history once.  Every input is checked before the history changes; a call that returns an
+ * error leaves it as it was.  wva_saturation_v2 / wva_pipeline_v2 may then run as often as the caller likes. */
+int32_t wva_k2_resolve(wva_k2_history* h, const wva_k2_in* in, const wva_k2_out* out);
+/* Every key (wva_k2_history_keys of them): history group, accelerator id, bucket, count (0..10), values [K*10] oldest
+ * first (zeros past count). */
+int32_t wva_k2_history_export(wva_k2_history* h, int32_t* hg, int32_t* acc, int32_t* bucket, int32_t* count, double* values);
+/* Replaces the whole history with n keys in the export format (keys not listed start empty).  A key not registered,
+ * listed twice, a bucket outside 0..2 or a count outside 0..10 is WVA_ERR_ARG and changes nothing. */
+int32_t wva_k2_history_import(wva_k2_history* h, int64_t n, const int32_t* hg, const int32_t* acc, const int32_t* bucket,
+                              const int32_t* count, const double* values);
 
 /* ---- host memory ----------------------------------------------------------- */
 /* Page-locked host buffers for the caller's SoA arrays (the collector writes its batch straight into them): every

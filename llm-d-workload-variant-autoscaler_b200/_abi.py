@@ -295,6 +295,60 @@ def make_saturation_v2(d: dict):
     return ist, ost, keep, out
 
 
+# ---- k2 priority chain with its rolling history ----------------------------------------------------------------------
+class K2In(C.Structure):
+    _fields_ = [("n_model_groups", C.c_int64), ("n_replicas", C.c_int64), ("model_replica_off", _i32p),
+                ("rep_total_kv_tokens", _i64p), ("rep_tokens_in_use", _i64p), ("rep_queue_length", _i64p),
+                ("rep_avg_input_tokens", _f64p), ("rep_avg_output_tokens", _f64p), ("rep_accelerator", _i32p),
+                ("rep_slot", _i32p), ("rep_out_pos", _i32p), ("n_out", C.c_int64),
+                ("slot_max_batched_tokens", _i64p), ("slot_max_num_seqs", _i64p),
+                ("cfg_queue_threshold", _f64p), ("cfg_kv_threshold", _f64p)]
+
+
+class K2Out(C.Structure):
+    _fields_ = [("rep_k2", _i64p), ("rep_effective", _i64p), ("out_rep_k2", _i64p), ("slot_last_rep", _i32p),
+                ("slot_effective", _i64p)]
+
+
+# name -> (dtype, extent): G model groups, P replicas, S store slots
+K2_IN = {"model_replica_off": (np.int32, "G1"), "rep_total_kv_tokens": (np.int64, "P"), "rep_tokens_in_use": (np.int64, "P"),
+         "rep_queue_length": (np.int64, "P"), "rep_avg_input_tokens": (np.float64, "P"),
+         "rep_avg_output_tokens": (np.float64, "P"), "rep_accelerator": (np.int32, "P"), "rep_slot": (np.int32, "P"),
+         "rep_out_pos": (np.int32, "P"), "slot_max_batched_tokens": (np.int64, "S"), "slot_max_num_seqs": (np.int64, "S"),
+         "cfg_queue_threshold": (np.float64, "G"), "cfg_kv_threshold": (np.float64, "G")}
+K2_OUT = {"rep_k2": (np.int64, "P"), "rep_effective": (np.int64, "P"), "out_rep_k2": (np.int64, "N"),
+          "slot_last_rep": (np.int32, "S"), "slot_effective": (np.int64, "S")}
+
+
+def make_k2(d: dict, n_slots: int):
+    """d: the K2_IN columns (rep_out_pos may be absent or None; then n_out is ignored) -> (in, out, keep-alive, outputs)."""
+    G, P = len(d["model_replica_off"]) - 1, len(d["rep_total_kv_tokens"])
+    has_pos = d.get("rep_out_pos") is not None
+    N = int(d.get("n_out", 0)) if has_pos else 0
+    n = {"G": G, "G1": G + 1, "P": P, "S": n_slots, "N": N}
+    ist, ost, keep, out = K2In(), K2Out(), [], {}
+    ist.n_model_groups, ist.n_replicas, ist.n_out = G, P, N
+    for name, (dt, dim) in K2_IN.items():
+        if name == "rep_out_pos" and not has_pos:
+            setattr(ist, name, None)
+            continue
+        a = np.ascontiguousarray(d[name], dtype=dt).reshape(-1)
+        if a.size != n[dim]:
+            raise ValueError(f"{name}: expected {n[dim]} elements, got {a.size}")
+        if a.size == 0:
+            a = np.zeros(1, dt)
+        keep.append(a)
+        setattr(ist, name, ptr(a))
+    for name, (dt, dim) in K2_OUT.items():
+        if name == "out_rep_k2" and not has_pos:
+            setattr(ost, name, None)
+            continue
+        a = np.zeros(max(n[dim], 1), dtype=dt)
+        setattr(ost, name, ptr(a))
+        out[name] = a[:n[dim]]
+    return ist, ost, keep, out
+
+
 # ---- ingest ------------------------------------------------------------------------------------------------------------
 class IngestColumns(C.Structure):
     _fields_ = [("n_slots", C.c_int64), ("n_variants", C.c_int64), ("n_models", C.c_int64),

@@ -14,6 +14,7 @@
 #include "saturation_kernel.cuh"
 #include "limiter_kernel.cuh"
 #include "pipeline_v2_kernel.cuh"
+#include "k2_history_kernel.cuh"
 #include "overflow_slow_kernel.cuh"
 #include "greedy_solve.cuh"
 #include "greedy_sweep.cuh"
@@ -822,3 +823,4 @@ int32_t wva_get_solution(wva_ctx* ctx, wva_solution* out) {
 #include "capi_aux.inl"
 #include "comm.inl"
 #include "ingest.inl"
+#include "k2_history.inl"

@@ -99,6 +99,13 @@ def load_library():
     L.wva_cost_aware_optimize.argtypes = [ctxp, C.c_int64, C.c_int64] + [C.c_void_p] * 8
     L.wva_enforce.argtypes = [ctxp, C.c_int64, C.c_int64] + [C.c_void_p] * 8
     L.wva_pipeline_v2.argtypes = [ctxp, C.POINTER(abi.SaturationV2In)] + [C.c_void_p] * 5 + [C.POINTER(abi.SaturationV2Out), C.c_void_p, C.c_void_p]
+    L.wva_k2_history_create.argtypes = [ctxp, C.c_int64, C.c_int64, C.c_int64] + [C.c_void_p] * 4 + [C.POINTER(ctxp)]
+    L.wva_k2_history_destroy.argtypes = [ctxp]
+    L.wva_k2_history_keys.argtypes = [ctxp]
+    L.wva_k2_history_keys.restype = C.c_int64
+    L.wva_k2_resolve.argtypes = [ctxp, C.POINTER(abi.K2In), C.POINTER(abi.K2Out)]
+    L.wva_k2_history_export.argtypes = [ctxp] + [C.c_void_p] * 5
+    L.wva_k2_history_import.argtypes = [ctxp, C.c_int64] + [C.c_void_p] * 5
     L.wva_host_alloc.argtypes = [C.c_size_t, C.POINTER(C.c_void_p)]
     L.wva_host_free.argtypes = [C.c_void_p]
     L.wva_last_timing.argtypes = [ctxp, C.POINTER(abi.Timing)]
@@ -115,7 +122,9 @@ EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_l
            "wva_microbench_fp64", "wva_set_optimizer", "wva_set_capacity", "wva_comm_unique_id", "wva_comm_init_rank",
            "wva_comm_shard", "wva_group_create", "wva_group_destroy", "wva_group_size", "wva_group_ctx",
            "wva_group_optimize", "wva_group_saturation_v1", "wva_ingest_create", "wva_ingest_destroy", "wva_ingest_begin",
-           "wva_ingest_write", "wva_ingest_commit", "wva_ingest_create_decisions"]
+           "wva_ingest_write", "wva_ingest_commit", "wva_ingest_create_decisions", "wva_k2_history_create",
+           "wva_k2_history_destroy", "wva_k2_history_keys", "wva_k2_resolve", "wva_k2_history_export",
+           "wva_k2_history_import"]
 
 
 def comm_unique_id() -> bytes:
@@ -401,6 +410,60 @@ class Engine:
         a, b = C.c_double(), C.c_double()
         self._check(self.lib.wva_microbench_fp64(self.ctx, C.byref(a), C.byref(b)), "wva_microbench_fp64")
         return a.value, b.value
+
+
+class K2History:
+    """wva_k2_history: the V2 analyzer's k2 priority chain (computeK2) with its rolling history resident on the device
+    (include/wva_b200.h).  Registry, all int32: hg_model_off [H+1] / hg_models [G] (history group = modelID -> its model
+    groups in visiting order), hg_acc_off [H+1] / hg_acc (its distinct accelerator ids), n_slots store slots.  A registry
+    change = export(), a new K2History, import_()."""
+
+    def __init__(self, engine: Engine, hg_model_off, hg_models, hg_acc_off, hg_acc, n_slots: int):
+        self.engine, self.lib, self.h = engine, engine.lib, C.c_void_p()
+        arr = lambda a: np.ascontiguousarray(a, np.int32).reshape(-1)
+        mo, m, ao, a = arr(hg_model_off), arr(hg_models), arr(hg_acc_off), arr(hg_acc)
+        p = lambda x: x.ctypes.data if x.size else None
+        self.H, self.G, self.n_slots = len(mo) - 1, len(m), int(n_slots)
+        engine._check(self.lib.wva_k2_history_create(engine.ctx, self.H, self.G, self.n_slots, p(mo), p(m), p(ao), p(a),
+                                                     C.byref(self.h)), "wva_k2_history_create")
+        self.K = int(self.lib.wva_k2_history_keys(self.h))
+
+    def close(self):
+        if self.h:
+            self.lib.wva_k2_history_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def resolve(self, d: dict) -> dict:
+        """One cycle (abi.K2_IN columns, optional rep_out_pos + n_out) -> rep_k2, rep_effective, slot_last_rep,
+        slot_effective (and out_rep_k2 with rep_out_pos).  Appends to the history once."""
+        ist, ost, keep, out = abi.make_k2(d, self.n_slots)
+        self.engine._check(self.lib.wva_k2_resolve(self.h, C.byref(ist), C.byref(ost)), "wva_k2_resolve")
+        return out
+
+    def export(self) -> dict:
+        """every key: hg, acc, bucket, count [K] and values [K, 10] oldest first"""
+        K = max(self.K, 1)
+        out = {k: np.zeros(K, np.int32) for k in ("hg", "acc", "bucket", "count")}
+        out["values"] = np.zeros((K, 10), np.float64)
+        self.engine._check(self.lib.wva_k2_history_export(self.h, *(out[k].ctypes.data for k in ("hg", "acc", "bucket", "count", "values"))),
+                           "wva_k2_history_export")
+        return {k: v[:self.K] for k, v in out.items()}
+
+    def import_(self, e: dict):
+        """replace the history with the keys of `e` (export format; keys not listed start empty)"""
+        cols = [np.ascontiguousarray(e[k], np.int32).reshape(-1) for k in ("hg", "acc", "bucket", "count")]
+        vals = np.ascontiguousarray(e["values"], np.float64).reshape(-1, 10)
+        n = len(cols[0])
+        if any(len(c) != n for c in cols) or len(vals) != n:
+            raise ValueError("import: columns of different lengths")
+        p = lambda x: x.ctypes.data if x.size else None
+        self.engine._check(self.lib.wva_k2_history_import(self.h, n, *(p(c) for c in cols), p(vals)), "wva_k2_history_import")
 
 
 class Ingest:

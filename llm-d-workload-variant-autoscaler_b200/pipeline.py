@@ -229,6 +229,7 @@ def ingest_decisions(ing, models, variant_names, accelerator_names, limiter_name
 # ======================================================================================================================
 ROLLING_AVERAGE_WINDOW = 10        # saturation_v2/constants.go RollingAverageWindowSize
 SHORT_OUTPUT, MEDIUM_OUTPUT = 100, 500
+BUCKETS = ("short", "medium", "long")     # output-length buckets, in the device history's bucket order
 COMPAT_FIELDS = ("GpuMemoryUtilization", "BlockSize", "KvCacheDtype", "TensorParallelSize", "NumGpuBlocksOverride",
                  "EffectiveMaxBatchedTokens")   # VLLMEngineParams.IsCapacityCompatible (deployment_parser.go:225-235)
 
@@ -290,13 +291,105 @@ class SaturationAnalyzerV2:
     :218-262), the capacity store and the zero-replica estimates (:317-324, :351-415) — and feeds the device the
     per-replica k2 and per-variant fallback capacity; all arithmetic on the metrics is `wva_saturation_v2`."""
 
-    def __init__(self, engine, store: CapacityKnowledgeStore | None = None):
+    def __init__(self, engine, store: CapacityKnowledgeStore | None = None, device_history: bool = False):
+        """device_history: keep the rolling k2 history on the device (`engine.K2History`) and resolve the k2 chain and
+        the per-slot store updates there (`wva_k2_resolve`) instead of in the host chain below."""
         self.engine = engine
         self.store = store or CapacityKnowledgeStore()
-        self.history = {}          # "model|accelerator|bucket" -> list of float (window 10)
+        self.history = {}          # "model|accelerator|bucket" -> list of float (window 10); host chain only
+        self.k2 = None             # the device history (device_history=True), rebuilt when its registry changes
+        self.device_history = device_history
+        self._k2_reg = None        # (modelID per input, {modelID: accelerator names}, n_slots) of self.k2
+        self._k2_hgs = []          # modelID per history group of self.k2
+        self._acc_id, self._slot = {}, {}   # accelerator name -> id; (namespace, model, variant) -> store slot
 
     def name(self):
         return "saturation-token-based"
+
+    def close(self):
+        if self.k2 is not None:
+            self.k2.close()
+            self.k2 = None
+
+    # -- the device history -------------------------------------------------------------------------------------------
+    def history_state(self) -> dict:
+        """the rolling history as {"model|accelerator|bucket": [values oldest first]} (keys with values only)"""
+        if not self.device_history:
+            return {k: list(v) for k, v in self.history.items() if v}
+        if self.k2 is None:
+            return {}
+        e, names = self.k2.export(), {i: n for n, i in self._acc_id.items()}
+        return {"%s|%s|%s" % (self._k2_hgs[int(e["hg"][k])], names[int(e["acc"][k])], BUCKETS[int(e["bucket"][k])]):
+                [float(x) for x in e["values"][k, :int(e["count"][k])]] for k in range(len(e["hg"])) if e["count"][k] > 0}
+
+    def _k2_registry(self, inputs):
+        """the handle for this batch: its model groups are the inputs in list order, its history groups every modelID of
+        the batch and every modelID the history already holds.  A new registry = export, create, import."""
+        models = tuple(inp.get("ModelID", "") for inp in inputs)
+        accs = {}
+        for m, inp in zip(models, inputs):
+            for rm in inp.get("ReplicaMetrics", []) or []:
+                accs.setdefault(m, {})[rm.get("AcceleratorName", "")] = None
+                self._slot.setdefault((inp.get("Namespace", ""), m, rm["VariantName"]), len(self._slot))
+            for s in inp.get("VariantStates", []) or []:
+                self._slot.setdefault((inp.get("Namespace", ""), m, s["VariantName"]), len(self._slot))
+        if self.k2 is not None and self._k2_reg[0] == models and len(self._slot) <= self._k2_reg[2] and \
+                all(a in self._k2_reg[1].get(m, ()) for m, s in accs.items() for a in s):
+            return
+        old = self.history_state()
+        for key in old:
+            m, a, _ = key.rsplit("|", 2)
+            accs.setdefault(m, {})[a] = None
+        for m, s in (self._k2_reg[1] if self._k2_reg else {}).items():
+            for a in s:
+                accs.setdefault(m, {})[a] = None
+        hgs = list(dict.fromkeys(models + tuple(accs)))
+        mo, mg, ao, ai = [0], [], [0], []
+        for m in hgs:
+            mg += [i for i, x in enumerate(models) if x == m]
+            mo.append(len(mg))
+            ai += [self._acc_id.setdefault(a, len(self._acc_id)) for a in accs.get(m, {})]
+            ao.append(len(ai))
+        self.close()
+        n_slots = max(len(self._slot), 1)
+        from .engine import K2History
+        self.k2 = K2History(self.engine, mo, mg, ao, ai, n_slots)
+        self._k2_reg, self._k2_hgs = (models, {m: tuple(accs.get(m, {})) for m in hgs}, n_slots), hgs
+        rows = []
+        for key, vals in old.items():
+            m, a, b = key.rsplit("|", 2)
+            rows.append((hgs.index(m), self._acc_id[a], BUCKETS.index(b), len(vals), vals + [0.0] * (10 - len(vals))))
+        if rows:
+            self.k2.import_({"hg": [r[0] for r in rows], "acc": [r[1] for r in rows], "bucket": [r[2] for r in rows],
+                             "count": [r[3] for r in rows], "values": [r[4] for r in rows]})
+
+    def _k2_device(self, inputs, pos_of_all, n_out):
+        """wva_k2_resolve over the batch: rep_k2 in the wva_saturation_v2 layout, and the per-slot last data replica"""
+        self._k2_registry(inputs)
+        cols = {k: [] for k in ("rep_total_kv_tokens", "rep_tokens_in_use", "rep_queue_length", "rep_avg_input_tokens",
+                                "rep_avg_output_tokens", "rep_accelerator", "rep_slot", "rep_out_pos")}
+        off, qthr, kvthr, rows = [0], [], [], []
+        S = self._k2_reg[2]
+        sB, sS = [0] * S, [0] * S
+        for inp, pos_of in zip(inputs, pos_of_all):
+            ns, model, c = inp.get("Namespace", ""), inp.get("ModelID", ""), inp["Config"]
+            for i, rm in enumerate(inp.get("ReplicaMetrics", []) or []):
+                s = self._slot[(ns, model, rm["VariantName"])]
+                cols["rep_total_kv_tokens"].append(int(rm.get("TotalKvCapacityTokens", 0)))
+                cols["rep_tokens_in_use"].append(int(rm.get("TokensInUse", 0)))
+                cols["rep_queue_length"].append(int(rm.get("QueueLength", 0)))
+                cols["rep_avg_input_tokens"].append(float(rm.get("AvgInputTokens", 0.0)))
+                cols["rep_avg_output_tokens"].append(float(rm.get("AvgOutputTokens", 0.0)))
+                cols["rep_accelerator"].append(self._acc_id[rm.get("AcceleratorName", "")])
+                cols["rep_slot"].append(s)
+                cols["rep_out_pos"].append(pos_of.get(i, -1))
+                rec = self.store.get(ns, model, rm["VariantName"])        # params as of the start of the cycle
+                p = (rec.get("VLLMParams") if rec else None) or {}
+                sB[s], sS[s] = int(p.get("EffectiveMaxBatchedTokens", 0)), int(p.get("MaxNumSeqs", 0))
+            off.append(len(cols["rep_slot"]))
+            qthr.append(float(c.get("QueueLengthThreshold", 0.0))); kvthr.append(float(c.get("KvCacheThreshold", 0.0)))
+        return self.k2.resolve(dict(cols, model_replica_off=off, n_out=n_out, slot_max_batched_tokens=sB,
+                                    slot_max_num_seqs=sS, cfg_queue_threshold=qthr, cfg_kv_threshold=kvthr)), off
 
     # -- caller-side state machines -----------------------------------------------------------------------------------
     def _k2(self, model_id, rm, queue_threshold, params):
@@ -348,7 +441,7 @@ class SaturationAnalyzerV2:
         rep = {k: [] for k in ("tk", "tu", "ql", "ai", "ao", "hr", "k2")}
         order, vcur, vpen, vfb, cfg = [], [], [], [], ([], [], [])
         qs, qb, any_queue = [], [], False
-        meta = []
+        meta, pos_all = [], []
         for inp in inputs:
             model, ns, c = inp.get("ModelID", ""), inp.get("Namespace", ""), inp["Config"]
             rms, states = inp.get("ReplicaMetrics", []) or [], inp.get("VariantStates", []) or []
@@ -357,7 +450,7 @@ class SaturationAnalyzerV2:
             # phase 1 in slice order: the k2 chain mutates the history, the store is updated with live data
             k2_of, eff_of = {}, {}
             for i, rm in enumerate(rms):
-                if int(rm.get("TotalKvCapacityTokens", 0)) <= 0:
+                if self.device_history or int(rm.get("TotalKvCapacityTokens", 0)) <= 0:
                     continue
                 rec = self.store.get(ns, model, rm["VariantName"])
                 params = rec.get("VLLMParams") if rec else None
@@ -380,6 +473,7 @@ class SaturationAnalyzerV2:
             # replicas of variants without a state do not reach any VariantCapacity but count in the workload averages:
             # keep them in the slice order with a trailing phantom variant only if needed (not produced by the collector)
             order += [pos_of[i] for i in range(len(rms)) if i in pos_of]
+            pos_all.append(pos_of)
             # per-model context for the zero-replica fallbacks, resolved after the live capacities reached the store
             ai = ao = 0.0; cnt = 0                                  # computeModelWorkloadAverages :438-455
             for rm in rms:
@@ -404,21 +498,32 @@ class SaturationAnalyzerV2:
                  rep_avg_output_tokens=rep["ao"], rep_prefix_hit_rate=rep["hr"], rep_k2=rep["k2"], rep_slice_order=order,
                  var_current=vcur, var_pending=vpen, var_fallback_capacity=vfb, cfg_kv_threshold=cfg[0], cfg_scale_up_threshold=cfg[1],
                  cfg_scale_down_boundary=cfg[2], sched_queue_size=qs if any_queue else None, sched_queue_bytes=qb if any_queue else None)
+        if self.device_history:
+            k2out, k2off = self._k2_device(inputs, pos_all, len(rep["tk"]))
+            d["rep_k2"] = k2out["out_rep_k2"]
         out = self.engine.saturation_v2(d)
         # the live capacities go into the store (analyzer.go:184-196, VLLMParams preserved) ...
         for mi, (inp, names, by_var, accel, cost, gpus, avg_of) in enumerate(meta):
             rms = inp.get("ReplicaMetrics", []) or []
             ns, model = inp.get("Namespace", ""), inp.get("ModelID", "")
+
+            def update(v, i, eff):
+                old = self.store.get(ns, model, v)
+                self.store.update(ns, model, v, {"AcceleratorName": rms[i].get("AcceleratorName", ""), "GpuCount": gpus.get(v, 0),
+                                                 "NumGpuBlocks": int(rms[i].get("NumGpuBlocks", 0)), "BlockSize": int(rms[i].get("BlockSize", 0)),
+                                                 "TotalKvCapacityTokens": int(rms[i]["TotalKvCapacityTokens"]), "EffectiveCapacity": eff,
+                                                 "VLLMParams": old.get("VLLMParams") if old else None, "LearnedFrom": "live"})
             for k, v in enumerate(names):
                 vi = mvo[mi] + k
+                if self.device_history:                     # once per slot: its last data replica of the cycle
+                    s = self._slot[(ns, model, v)]
+                    last = int(k2out["slot_last_rep"][s])
+                    if last >= 0:
+                        update(v, last - k2off[mi], int(k2out["slot_effective"][s]))
+                    continue
                 for j, i in enumerate(by_var.get(v, [])):
                     if int(rms[i].get("TotalKvCapacityTokens", 0)) > 0:
-                        old = self.store.get(ns, model, v)
-                        self.store.update(ns, model, v, {"AcceleratorName": rms[i].get("AcceleratorName", ""), "GpuCount": gpus.get(v, 0),
-                                                         "NumGpuBlocks": int(rms[i].get("NumGpuBlocks", 0)), "BlockSize": int(rms[i].get("BlockSize", 0)),
-                                                         "TotalKvCapacityTokens": int(rms[i]["TotalKvCapacityTokens"]),
-                                                         "EffectiveCapacity": int(out["rep_effective"][vro[vi] + j]),
-                                                         "VLLMParams": old.get("VLLMParams") if old else None, "LearnedFrom": "live"})
+                        update(v, i, int(out["rep_effective"][vro[vi] + j]))
         # ... before the variants without ready replicas look a capacity up (:317-324); those models are evaluated again
         any_fb = False
         for mi, (inp, names, by_var, accel, cost, gpus, avg_of) in enumerate(meta):
