@@ -109,6 +109,41 @@ __device__ __forceinline__ bool grid_setup(PairModel& m, const SysView& s, int s
   return true;
 }
 
+// model_finish(m, tabf, 1) with its two scans over the table spread over the warp's lanes: the same model.  mono is one
+// past the LAST descent !(tab[n-1] <= tab[n]) (where model_finish's scan from the top stops), a max over n; e1_ok needs
+// every entry to be an (E1) divisor, an and over n (model_finish checks the entries below mono and the two ends of the
+// non-decreasing rest, which bound every entry between them: e1_divisor is an interval test).  Run by one lane, the
+// scan is N dependent shared-memory loads per pair, a long stretch of the warp's time when the chains are short.
+__device__ __forceinline__ void grid_model_finish(PairModel& m, const float* tabf) {
+  const int lane = threadIdx.x & 31;
+  int desc = 0;
+  bool e1 = true;
+  for (int n = lane; n < m.N; n += 32) {
+    const float cur = tabf[n];
+    e1 = e1 && e1_divisor(cur);
+    if (n > 0 && !(tabf[n - 1] <= cur)) desc = n;
+  }
+  m.tab = tabf; m.stride = 1;
+  const float rl = tabf[m.N - 1];
+  model_set_range(m, tabf[0], rl);
+  m.mono = __reduce_max_sync(0xffffffffu, desc);
+  m.e1_ok = __all_sync(0xffffffffu, e1) && rate_den_ok(rate_den(rate_coef(m), (float)m.N));
+  m.mu_last = (double)rl;
+  m.r_last = rcp_f32den(rl, m.mu_last);
+}
+
+// Phase profile of the main pass (tools/perf_grid_phases.py): built with -DWVA_GRID_PHASES, lane 0 of every warp adds
+// its clock64() cycles of the pair setup and head table, of the chain solves and of the whole loop, and its solves and
+// states (those of a pair's first round apart), to g_grid_phase (read by wva_grid_phases).  The product build compiles
+// none of it.
+#ifdef WVA_GRID_PHASES
+enum { GPH_TABLE, GPH_CHAIN, GPH_TOTAL, GPH_SOLVES, GPH_STATES, GPH_STATES0, GPH_N };
+__device__ unsigned long long g_grid_phase[GPH_N];
+#define GRID_PH(...) __VA_ARGS__
+#else
+#define GRID_PH(...)
+#endif
+
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, WARPS == 8 ? 2 : 1)
 grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax, GridCounters* ctr, GridDefer df,
@@ -119,8 +154,10 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
   double2* tab = smem_grid + (size_t)warp * nmax;
   float* tabf = (float*)(smem_grid + (size_t)WARPS * nmax) + (size_t)warp * nmax;
   unsigned long long my_solves = 0, my_states = 0, my_s0 = 0, my_sr = 0, my_rounds = 0;
+  GRID_PH(long long ph_table = 0, ph_chain = 0; unsigned long long ph_states0 = 0; const long long ph_start = clock64();)
 
   while (true) {
+    GRID_PH(const long long ph_t0 = clock64();)
     unsigned long long pair = 0;
     if (lane == 0) pair = atomicAdd(&ctr->next_pair, 1ull);
     pair = __shfl_sync(full, pair, 0);
@@ -141,6 +178,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
         if (out.tput) out.tput[obase + r] = 0.0f;
       }
       if (out.frontier && lane == 0) out.frontier[pair] = 0;
+      GRID_PH(ph_table += clock64() - ph_t0;)
       continue;
     }
     __syncwarp();
@@ -151,13 +189,14 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
       tab[n] = make_double2(mu, rcp_f32den(mu32, mu));
     }
     __syncwarp();
-    model_finish(m, tabf, 1);
+    grid_model_finish(m, tabf);
     const float lambda_tps = f_mul(m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));
     int front = 0x7fffffff;
     const bool deferring = df.side != nullptr && pair < 0xffffffffull;
     bool saved = false;                                   // the pair's model is written when its first level is deferred
     const float mu_last_f = (float)m.mu_last;
     bool first_round = true;
+    GRID_PH(ph_table += clock64() - ph_t0;)
 
     // Two levels per lane and round (r0 + lane + 1 and r0 + 32 + lane + 1): the two chains of a lane share every table
     // load and give the FP64 pipe two independent dependency chains; half as many rounds (the chains of a round are ~20
@@ -223,6 +262,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
       SolveStats st[2];
       int sv = 0;
       bool bad = false;
+      GRID_PH(const long long ph_c = clock64();)
       // a pair with a service rate outside the (E1) divisor range takes the per-lane chain below for every level
       if (!m.e1_ok) bad = here[0] || here[1];
       else if (__any_sync(full, here[0] || here[1])) lockstep_solve_inl<2, WarpTable>(m, WarpTable{tab}, lambda, here, st, sv, bad);
@@ -231,6 +271,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
         int mxs = (here[0] || here[1]) ? sv : 0;
         for (int o = 16; o; o >>= 1) mxs = max(mxs, __shfl_xor_sync(full, mxs, o));
         if (lane == 0) { if (first_round) my_s0 += 32ull * mxs; else my_sr += 32ull * mxs; my_rounds++; }
+        GRID_PH(if (first_round && (here[0] || here[1])) ph_states0 += (unsigned long long)sv;)
         first_round = false;
       }
       if (bad) {
@@ -247,6 +288,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
             if (ovf[c]) grid_overflow_push(ol, ctr, obase + (size_t)(r[c] - 1));
           }
       }
+      GRID_PH(__syncwarp(); ph_chain += clock64() - ph_c;)
 #pragma unroll
       for (int c = 0; c < 2; c++) {
         if (in_range[c] && !defer[c] && !ovf[c]) {
@@ -276,6 +318,17 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
     atomicAdd(&ctr->solves, my_solves); atomicAdd(&ctr->states, my_states);
     atomicAdd(&ctr->slots0, my_s0); atomicAdd(&ctr->slots_rest, my_sr); atomicAdd(&ctr->rounds, my_rounds);
   }
+#ifdef WVA_GRID_PHASES
+  for (int o = 16; o; o >>= 1) ph_states0 += __shfl_down_sync(full, ph_states0, o);
+  if (lane == 0) {
+    atomicAdd(&g_grid_phase[GPH_TABLE], (unsigned long long)ph_table);
+    atomicAdd(&g_grid_phase[GPH_CHAIN], (unsigned long long)ph_chain);
+    atomicAdd(&g_grid_phase[GPH_TOTAL], (unsigned long long)(clock64() - ph_start));
+    atomicAdd(&g_grid_phase[GPH_SOLVES], my_solves);
+    atomicAdd(&g_grid_phase[GPH_STATES], my_states);
+    atomicAdd(&g_grid_phase[GPH_STATES0], ph_states0);
+  }
+#endif
 }
 
 // The deferred levels, sorted by length class: lane per (pair, level), 32 different pairs per warp.
