@@ -644,6 +644,98 @@ int32_t wva_k2_history_export(wva_k2_history* h, int32_t* hg, int32_t* acc, int3
 int32_t wva_k2_history_import(wva_k2_history* h, int64_t n, const int32_t* hg, const int32_t* acc, const int32_t* bucket,
                               const int32_t* count, const double* values);
 
+/* ---- V2 ingest: metric batch -> V2 decisions in two graph launches around the host capacity store -------------------- */
+/*
+ * The V2 engine's cycle (optimizeV2, internal/engines/saturation/engine.go:397-488) from the six Prometheus vectors of
+ * CollectReplicaMetrics (internal/collector/replica_metrics.go:78-403) to the final VariantDecisions, with the same
+ * registry as wva_ingest (CSR model -> variant -> pod slot, the slots of a variant in ascending pod-name order: that
+ * order is the ReplicaMetrics slice order of the model, variant after variant, the canonical stand-in for the
+ * reference's `range podData` map order).  The capacity knowledge store stays with the caller, so a cycle is
+ *   begin -> write (samples) + the per-cycle columns -> wva_ingest_v2_analyze -> host step -> wva_ingest_v2_decide.
+ *
+ * analyze (one graph launch): H2D of the column arena; per pod slot the replica fields (a pod reports iff it has a KV
+ * or a queue sample, the missing one reads 0; queue = Go's int(float64); TotalKvCapacityTokens = blocks * size with
+ * hasCacheConfig, INT64_MAX on overflow, else 0; TokensInUse = clamp(math.Round(kv * total), 0, total) converted as
+ * Go's int64(float64)); the reporting pods packed per variant; the k2 chain of wva_k2_resolve against the handle's
+ * history (model group m of the history = model m here); D2H of the per-slot store updates, the variants without a
+ * replica with capacity data and the model workload averages (computeModelWorkloadAverages, analyzer.go:438-455).
+ * The registry checks of the k2 chain are made once at create; if the chain's error word is set anyway, the history is
+ * left as it was (the kernels test it on the device) and analyze returns WVA_ERR_ARG.
+ *
+ * host step (the caller, between the launches): the store updates once per store slot with slot_last_rep >= 0
+ * (analyzer.go:184-196, last write wins), then var_fallback_capacity for the variants with var_no_data (:317-415).
+ *
+ * Every column but var_fallback_capacity goes up with analyze: only var_fallback_capacity may change between analyze
+ * and decide (a write to another column in between is not seen by decide).
+ *
+ * decide (one graph launch): H2D of var_fallback_capacity; SaturationAnalyzer.Analyze -> CostAwareOptimizer.Optimize
+ * -> Enforcer.EnforcePolicy (the kernels of wva_pipeline_v2) for every model with a reporting pod (the others make no
+ * ModelScalingRequest: prepareModelData returns nil, engine.go:738-742); D2H of the results.  The optimizer and the
+ * enforcer see a variant's cost only when it has a reporting pod (the VariantCapacity's Cost is 0 otherwise).
+ * `res` arrays are valid after the launch that fills them, until the next one.  Registry change = destroy + create.
+ */
+typedef struct wva_ingest_v2 wva_ingest_v2;
+enum { WVA_VEC_AVG_OUTPUT_TOKENS = 2, WVA_VEC_AVG_INPUT_TOKENS = 3, WVA_VEC_PREFIX_CACHE_HIT_RATE = 4 };
+#define WVA_CACHE_LABEL_ABSENT INT64_MIN     /* a cache_config_info label that is absent or does not parse as int64 */
+typedef struct wva_ingest_v2_columns { /* page-locked host memory owned by the wva_ingest_v2; written every cycle   */
+  int64_t n_slots, n_variants, n_models, n_store_slots;
+  double* kv;                          /* [slots] KvCacheUsage sample                                               */
+  double* queue;                       /* [slots] queue-length sample                                               */
+  int64_t* num_gpu_blocks;             /* [slots] parsed cache_config_info labels                                   */
+  int64_t* block_size;                 /* [slots]                                                                   */
+  double* avg_output_tokens;           /* [slots] 0 until a finite sample arrives                                   */
+  double* avg_input_tokens;            /* [slots]                                                                   */
+  double* prefix_hit_rate;             /* [slots] 0 until a finite sample in [0, 1] arrives                         */
+  uint8_t* has;                        /* [slots] bit0 KV sample, bit1 queue sample, bit2 hasCacheConfig            */
+  double* var_cost;                    /* [V] ReplicaMetrics.Cost of the variant's pods                             */
+  int32_t* var_current; int32_t* var_pending;   /* [V] VariantReplicaState                                          */
+  int32_t* var_name_rank;              /* [V] rank of the variant's name among its model's (enforcer tie-break)     */
+  double* cfg_kv_threshold; double* cfg_queue_threshold;                 /* [M] SaturationScalingConfig            */
+  double* cfg_scale_up_threshold; double* cfg_scale_down_boundary;       /* [M]                                    */
+  uint8_t* mod_scale_to_zero_enabled; double* mod_request_count; uint8_t* mod_request_error;   /* [M] enforcer     */
+  int64_t* slot_max_batched_tokens;    /* [store slots] VLLMParams.EffectiveMaxBatchedTokens at the cycle's start  */
+  int64_t* slot_max_num_seqs;          /* [store slots] VLLMParams.MaxNumSeqs                                       */
+  double* var_fallback_capacity;       /* [V] written by the host step, read by decide                              */
+} wva_ingest_v2_columns;
+typedef struct wva_ingest_v2_results { /* page-locked host memory owned by the wva_ingest_v2                        */
+  /* analyze */
+  int32_t* variant_replica_off;        /* [V+1] replicas of variant v (its reporting pods, slot order)              */
+  int32_t* rep_pod;                    /* [slots] pod slot of replica r (first variant_replica_off[V] valid)        */
+  int64_t* rep_total_kv_tokens;        /* [slots] TotalKvCapacityTokens of replica r                                */
+  int32_t* slot_last_rep;              /* [store slots] last replica with capacity data of the slot, -1 = none      */
+  int64_t* slot_effective;             /* [store slots] its EffectiveCapacity                                       */
+  uint8_t* var_no_data;                /* [V] no replica with capacity data: the zero-replica fallback applies      */
+  uint8_t* mod_has_request;            /* [M] a pod of the model reported                                           */
+  double* mod_avg_input_tokens; double* mod_avg_output_tokens;           /* [M] workload averages                  */
+  /* decide */
+  int32_t* var_optimizer_target;       /* [V] CostAwareOptimizer's TargetReplicas, -1 without request               */
+  int32_t* var_target;                 /* [V] the enforced target, -1 without request                              */
+  int8_t* var_action;                  /* [V] sign(enforced target - current)                                       */
+  uint8_t* mod_enforced;               /* [M] EnforcePolicy's second result (0 without request)                     */
+  int32_t* var_ready;                  /* [V] as wva_saturation_v2_out                                              */
+  double* var_per_replica_capacity; double* var_total_capacity; double* var_total_demand; double* var_utilization;
+  double* mod_total_supply; double* mod_total_demand; double* mod_utilization;
+  double* mod_required_capacity; double* mod_spare_capacity;
+} wva_ingest_v2_results;
+/* var_accelerator [V]: accelerator id of the variant, registered for its model's history group; var_store_slot [V]:
+ * store slot of namespace|model|variant in [0, the history's n_slots).  The history's model groups must be the models. */
+int32_t wva_ingest_v2_create(wva_ctx* ctx, int64_t n_models, int64_t n_variants, int64_t n_slots,
+                             const int32_t* model_variant_off /* [M+1] */, const int32_t* variant_slot_off /* [V+1] */,
+                             const int32_t* var_accelerator, const int32_t* var_store_slot, wva_k2_history* h,
+                             wva_ingest_v2** out, wva_ingest_v2_columns* cols, wva_ingest_v2_results* res);
+int32_t wva_ingest_v2_destroy(wva_ingest_v2* ing);
+/* start of a cycle: no pod has a sample; avg_* and prefix_hit_rate read 0, the cache config is unset */
+int32_t wva_ingest_v2_begin(wva_ingest_v2* ing);
+/* one vector keyed by slot, in result order (WVA_VEC_*: a later sample of a pod overwrites an earlier one; a
+ * non-finite avg_* sample, or a hit rate that is non-finite or outside [0, 1], overwrites nothing); slot < 0 skipped */
+int32_t wva_ingest_v2_write(wva_ingest_v2* ing, int32_t which, int64_t n, const int32_t* slot, const double* value);
+/* cache_config_info: per sample the parsed labels (WVA_CACHE_LABEL_ABSENT leaves the value as it is); bit2 of `has`
+ * is set once both values are > 0 after a sample */
+int32_t wva_ingest_v2_write_cache_config(wva_ingest_v2* ing, int64_t n, const int32_t* slot, const int64_t* num_gpu_blocks,
+                                         const int64_t* block_size);
+int32_t wva_ingest_v2_analyze(wva_ingest_v2* ing);
+int32_t wva_ingest_v2_decide(wva_ingest_v2* ing);
+
 /* ---- host memory ----------------------------------------------------------- */
 /* Page-locked host buffers for the caller's SoA arrays (the collector writes its batch straight into them): every
  * entry point copies from / to such a buffer by DMA at link speed instead of through the driver's pageable staging

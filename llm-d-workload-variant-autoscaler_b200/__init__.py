@@ -8,7 +8,7 @@ or without a GPU raises.
 """
 from . import _abi, sharding, synth  # noqa: F401
 from . import engine, manager, pipeline  # noqa: F401
-from .engine import Engine, Group, Ingest, K2History, WvaError, comm_unique_id, lib_path, load_library, pinned_copy, pinned_empty  # noqa: F401
+from .engine import Engine, Group, Ingest, IngestV2, K2History, WvaError, comm_unique_id, lib_path, load_library, pinned_copy, pinned_empty  # noqa: F401
 from .manager import Manager, flatten_spec  # noqa: F401
 from .pipeline import (CapacityKnowledgeStore, CostAwareOptimizer, Enforcer, Limiter, SaturationAnalyzer,  # noqa: F401
-                       SaturationAnalyzerV2)
+                       SaturationAnalyzerV2, ingest_v2_decisions, optimize_v2)

@@ -375,3 +375,52 @@ class IngestDecisionResults(C.Structure):
 
 
 VEC_KV_CACHE_USAGE, VEC_QUEUE_LENGTH = 0, 1
+
+
+# ---- V2 ingest ---------------------------------------------------------------------------------------------------------
+class IngestV2Columns(C.Structure):
+    _fields_ = [("n_slots", C.c_int64), ("n_variants", C.c_int64), ("n_models", C.c_int64), ("n_store_slots", C.c_int64),
+                ("kv", _f64p), ("queue", _f64p), ("num_gpu_blocks", _i64p), ("block_size", _i64p),
+                ("avg_output_tokens", _f64p), ("avg_input_tokens", _f64p), ("prefix_hit_rate", _f64p), ("has", _u8p),
+                ("var_cost", _f64p), ("var_current", _i32p), ("var_pending", _i32p), ("var_name_rank", _i32p),
+                ("cfg_kv_threshold", _f64p), ("cfg_queue_threshold", _f64p), ("cfg_scale_up_threshold", _f64p),
+                ("cfg_scale_down_boundary", _f64p), ("mod_scale_to_zero_enabled", _u8p), ("mod_request_count", _f64p),
+                ("mod_request_error", _u8p), ("slot_max_batched_tokens", _i64p), ("slot_max_num_seqs", _i64p),
+                ("var_fallback_capacity", _f64p)]
+
+
+class IngestV2Results(C.Structure):
+    _fields_ = [("variant_replica_off", _i32p), ("rep_pod", _i32p), ("rep_total_kv_tokens", _i64p), ("slot_last_rep", _i32p),
+                ("slot_effective", _i64p), ("var_no_data", _u8p), ("mod_has_request", _u8p),
+                ("mod_avg_input_tokens", _f64p), ("mod_avg_output_tokens", _f64p),
+                ("var_optimizer_target", _i32p), ("var_target", _i32p), ("var_action", C.POINTER(C.c_int8)),
+                ("mod_enforced", _u8p), ("var_ready", _i32p), ("var_per_replica_capacity", _f64p),
+                ("var_total_capacity", _f64p), ("var_total_demand", _f64p), ("var_utilization", _f64p),
+                ("mod_total_supply", _f64p), ("mod_total_demand", _f64p), ("mod_utilization", _f64p),
+                ("mod_required_capacity", _f64p), ("mod_spare_capacity", _f64p)]
+
+
+VEC_AVG_OUTPUT_TOKENS, VEC_AVG_INPUT_TOKENS, VEC_PREFIX_CACHE_HIT_RATE = 2, 3, 4
+CACHE_LABEL_ABSENT = -(1 << 63)          # a cache_config_info label that is absent or does not parse
+
+# (name, dtype, dimension) of the V2 ingest arenas: S pod slots, V variants, M models, NS store slots
+INGEST_V2_COLUMNS = [("kv", np.float64, "S"), ("queue", np.float64, "S"), ("num_gpu_blocks", np.int64, "S"),
+                     ("block_size", np.int64, "S"), ("avg_output_tokens", np.float64, "S"),
+                     ("avg_input_tokens", np.float64, "S"), ("prefix_hit_rate", np.float64, "S"), ("has", np.uint8, "S"),
+                     ("var_cost", np.float64, "V"), ("var_current", np.int32, "V"), ("var_pending", np.int32, "V"),
+                     ("var_name_rank", np.int32, "V"), ("cfg_kv_threshold", np.float64, "M"),
+                     ("cfg_queue_threshold", np.float64, "M"), ("cfg_scale_up_threshold", np.float64, "M"),
+                     ("cfg_scale_down_boundary", np.float64, "M"), ("mod_scale_to_zero_enabled", np.uint8, "M"),
+                     ("mod_request_count", np.float64, "M"), ("mod_request_error", np.uint8, "M"),
+                     ("slot_max_batched_tokens", np.int64, "NS"), ("slot_max_num_seqs", np.int64, "NS"),
+                     ("var_fallback_capacity", np.float64, "V")]
+INGEST_V2_RESULTS = [("variant_replica_off", np.int32, "V1"), ("rep_pod", np.int32, "S"), ("rep_total_kv_tokens", np.int64, "S"),
+                     ("slot_last_rep", np.int32, "NS"), ("slot_effective", np.int64, "NS"), ("var_no_data", np.uint8, "V"),
+                     ("mod_has_request", np.uint8, "M"), ("mod_avg_input_tokens", np.float64, "M"),
+                     ("mod_avg_output_tokens", np.float64, "M"), ("var_optimizer_target", np.int32, "V"),
+                     ("var_target", np.int32, "V"), ("var_action", np.int8, "V"), ("mod_enforced", np.uint8, "M"),
+                     ("var_ready", np.int32, "V"), ("var_per_replica_capacity", np.float64, "V"),
+                     ("var_total_capacity", np.float64, "V"), ("var_total_demand", np.float64, "V"),
+                     ("var_utilization", np.float64, "V"), ("mod_total_supply", np.float64, "M"),
+                     ("mod_total_demand", np.float64, "M"), ("mod_utilization", np.float64, "M"),
+                     ("mod_required_capacity", np.float64, "M"), ("mod_spare_capacity", np.float64, "M")]

@@ -824,3 +824,4 @@ int32_t wva_get_solution(wva_ctx* ctx, wva_solution* out) {
 #include "comm.inl"
 #include "ingest.inl"
 #include "k2_history.inl"
+#include "ingest_v2.inl"

@@ -14,6 +14,8 @@
 //                       at most K2_SMEM_KEYS keys are staged in shared memory for the walk; larger groups work on them in
 //                       place in global memory.  Both run the same code on different pointers.
 //   k2_slot_kernel      per store slot: EffectiveCapacity of the slot's last data replica (atomicMax of its index).
+//   A caller that cannot read the error word back before the next launch (wva_ingest_v2's graph) passes it as `gate`:
+//   the resolve and slot kernels then return at once when it is set.
 //
 // Rings: per key `count` (0..10), `head` (index of the oldest value) and 10 float64 values; key index =
 // (hg_acc_off[h] + accelerator slot) * 3 + bucket.  A history group's keys are touched by its warp only.
@@ -40,6 +42,7 @@ struct K2In {
   const int *acc, *slot, *out_pos;
   const long long *slot_B, *slot_S;
   const double *q_thr, *kv_thr;
+  const int* gate;          // NULL, or the keys pass's error word: set = the resolve and slot kernels change nothing
 };
 struct K2Out { long long *rep_k2, *rep_eff, *out_k2; int* slot_last; long long* slot_eff; int* rep_key; int* err; };
 
@@ -86,6 +89,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32) k2_resolve_kernel(K2Reg reg, K2
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const unsigned before = (1u << lane) - 1u;
   double* obs_v = s_obs[wid];
+  if (in.gate && *in.gate) return;                                           // a rejected cycle leaves the history as it was
   for (int h = blockIdx.x * K2_WARPS + wid; h < reg.H; h += gridDim.x * K2_WARPS) {
     const int key0 = reg.hg_acc_off[h] * 3, nk = reg.hg_acc_off[h + 1] * 3 - key0;
     const bool staged = nk <= K2_SMEM_KEYS;
@@ -194,7 +198,8 @@ __global__ void __launch_bounds__(K2_WARPS * 32) k2_resolve_kernel(K2Reg reg, K2
   }
 }
 
-__global__ void k2_slot_kernel(int n_slots, const int* slot_last, const long long* rep_eff, long long* slot_eff) {
+__global__ void k2_slot_kernel(int n_slots, const int* slot_last, const long long* rep_eff, long long* slot_eff, const int* gate) {
+  if (gate && *gate) return;
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
     const int r = slot_last[s];
     slot_eff[s] = r >= 0 ? rep_eff[r] : 0;

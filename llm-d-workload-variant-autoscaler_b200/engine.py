@@ -80,6 +80,14 @@ def load_library():
     L.wva_ingest_begin.argtypes = [ctxp]
     L.wva_ingest_write.argtypes = [ctxp, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]
     L.wva_ingest_commit.argtypes = [ctxp]
+    L.wva_ingest_v2_create.argtypes = [ctxp, C.c_int64, C.c_int64, C.c_int64] + [C.c_void_p] * 4 + [ctxp, C.POINTER(ctxp),
+                                       C.POINTER(abi.IngestV2Columns), C.POINTER(abi.IngestV2Results)]
+    L.wva_ingest_v2_destroy.argtypes = [ctxp]
+    L.wva_ingest_v2_begin.argtypes = [ctxp]
+    L.wva_ingest_v2_write.argtypes = [ctxp, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]
+    L.wva_ingest_v2_write_cache_config.argtypes = [ctxp, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.wva_ingest_v2_analyze.argtypes = [ctxp]
+    L.wva_ingest_v2_decide.argtypes = [ctxp]
     L.wva_load_system.argtypes = [ctxp, C.POINTER(abi.System)]
     L.wva_calculate.argtypes = [ctxp]
     L.wva_solve.argtypes = [ctxp]
@@ -124,7 +132,8 @@ EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_l
            "wva_group_optimize", "wva_group_saturation_v1", "wva_ingest_create", "wva_ingest_destroy", "wva_ingest_begin",
            "wva_ingest_write", "wva_ingest_commit", "wva_ingest_create_decisions", "wva_k2_history_create",
            "wva_k2_history_destroy", "wva_k2_history_keys", "wva_k2_resolve", "wva_k2_history_export",
-           "wva_k2_history_import"]
+           "wva_k2_history_import", "wva_ingest_v2_create", "wva_ingest_v2_destroy", "wva_ingest_v2_begin",
+           "wva_ingest_v2_write", "wva_ingest_v2_write_cache_config", "wva_ingest_v2_analyze", "wva_ingest_v2_decide"]
 
 
 def comm_unique_id() -> bytes:
@@ -540,6 +549,75 @@ class Ingest:
         if self.h:
             self.lib.wva_ingest_destroy(self.h)
             self.h = None
+
+
+def _view(p, n, dt):
+    """numpy view of n elements of a library-owned page-locked array"""
+    if n == 0:
+        return np.zeros(0, dt)
+    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(n * np.dtype(dt).itemsize,)).view(dt)
+
+
+class IngestV2:
+    """wva_ingest_v2: the V2 reconcile cycle from metric batch to decisions in two graph launches around the host
+    capacity store (include/wva_b200.h).  registry: model_variant_off [M+1], variant_slot_off [V+1] (CSR model ->
+    variant -> pod slot, the slots of a variant in ascending pod-name order), var_accelerator [V] (accelerator ids of
+    `k2`'s registry), var_store_slot [V] (store slot of namespace|model|variant); `k2` = a K2History whose model groups
+    are the models (it must outlive this object).  A cycle: begin(), write() / write_cache_config() and the per-cycle
+    columns of `cols`, analyze(), the host step (writes cols["var_fallback_capacity"]), decide(); `res` holds the
+    results of the last launch."""
+
+    def __init__(self, engine: "Engine", model_variant_off, variant_slot_off, var_accelerator, var_store_slot, k2: K2History):
+        self.engine, self.lib, self.k2 = engine, engine.lib, k2
+        mvo = np.ascontiguousarray(model_variant_off, np.int32); vso = np.ascontiguousarray(variant_slot_off, np.int32)
+        acc = np.ascontiguousarray(var_accelerator, np.int32); sl = np.ascontiguousarray(var_store_slot, np.int32)
+        M, V, S = mvo.size - 1, vso.size - 1, int(vso[-1])
+        self.M, self.V, self.S, self.NS = M, V, S, k2.n_slots
+        self.model_variant_off, self.variant_slot_off, self.var_accelerator, self.var_store_slot = mvo, vso, acc, sl
+        self.h = C.c_void_p()
+        cst, rst = abi.IngestV2Columns(), abi.IngestV2Results()
+        p = lambda x: x.ctypes.data if x.size else None
+        engine._check(self.lib.wva_ingest_v2_create(engine.ctx, M, V, S, mvo.ctypes.data, vso.ctypes.data, p(acc), p(sl), k2.h,
+                                                    C.byref(self.h), C.byref(cst), C.byref(rst)), "wva_ingest_v2_create")
+        n = {"S": S, "V": V, "M": M, "NS": self.NS, "V1": V + 1}
+        self.cols = {k: _view(getattr(cst, k), n[d], dt) for k, dt, d in abi.INGEST_V2_COLUMNS}
+        self.res = {k: _view(getattr(rst, k), n[d], dt) for k, dt, d in abi.INGEST_V2_RESULTS}
+
+    def begin(self):
+        self.engine._check(self.lib.wva_ingest_v2_begin(self.h), "wva_ingest_v2_begin")
+
+    def write(self, which: int, slot, value):
+        sl = np.ascontiguousarray(slot, np.int32); va = np.ascontiguousarray(value, np.float64)
+        self.engine._check(self.lib.wva_ingest_v2_write(self.h, which, sl.size, sl.ctypes.data, va.ctypes.data), "wva_ingest_v2_write")
+
+    def write_cache_config(self, slot, num_gpu_blocks, block_size):
+        sl = np.ascontiguousarray(slot, np.int32)
+        b = np.ascontiguousarray(num_gpu_blocks, np.int64); s = np.ascontiguousarray(block_size, np.int64)
+        self.engine._check(self.lib.wva_ingest_v2_write_cache_config(self.h, sl.size, sl.ctypes.data, b.ctypes.data, s.ctypes.data),
+                           "wva_ingest_v2_write_cache_config")
+
+    def analyze(self):
+        """the first graph launch; analyze_ms = its device time (H2D + pack + k2 chain + D2H, CUDA events)"""
+        self.engine._check(self.lib.wva_ingest_v2_analyze(self.h), "wva_ingest_v2_analyze")
+        self.analyze_ms = float(self.engine.timing()["saturation_ms"])
+        return self.res
+
+    def decide(self):
+        """the second graph launch; decide_ms = its device time (H2D + analyzer + optimizer + enforcer + D2H)"""
+        self.engine._check(self.lib.wva_ingest_v2_decide(self.h), "wva_ingest_v2_decide")
+        self.decide_ms = float(self.engine.timing()["saturation_ms"])
+        return self.res
+
+    def close(self):
+        if self.h:
+            self.lib.wva_ingest_v2_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
 
 
 class Group:

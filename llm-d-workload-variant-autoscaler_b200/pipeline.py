@@ -259,21 +259,26 @@ def estimate_capacity_from_params(params, avg_in: float, avg_out: float) -> int:
 
 
 class CapacityKnowledgeStore:
-    """capacity_store.go: records keyed namespace|model|variant (insertion order = Go map stand-in for FindCompatible)."""
+    """capacity_store.go: records keyed namespace|model|variant (insertion order = Go map stand-in for FindCompatible).
+    Records are written through update() only: find_compatible visits a model's keys from an index update() keeps, so a
+    record placed into `records` directly is not seen by it."""
 
     def __init__(self):
         self.records = {}
+        self._of_model = {}        # model -> its keys in the records' insertion order (FindCompatible visits no other)
 
     def get(self, ns, model, variant):
         return self.records.get((ns, model, variant))
 
     def update(self, ns, model, variant, rec):
         self.records[(ns, model, variant)] = dict(rec)
+        self._of_model.setdefault(model, {})[(ns, model, variant)] = None
 
     def find_compatible(self, model, accelerator, gpu_count, params):
         best = None
-        for (ns, m, v), rec in self.records.items():
-            if m != model or rec.get("AcceleratorName") != accelerator or rec.get("GpuCount") != gpu_count:
+        for key in self._of_model.get(model, ()):
+            rec = self.records[key]
+            if rec.get("AcceleratorName") != accelerator or rec.get("GpuCount") != gpu_count:
                 continue
             p = rec.get("VLLMParams")
             if not p or not params or any(p.get(f) != params.get(f) for f in COMPAT_FIELDS):
@@ -431,6 +436,27 @@ class SaturationAnalyzerV2:
                 return float(bounded)
         return float(rec.get("EffectiveCapacity", 0))
 
+    # -- the host step around the analysis: store updates, then the zero-replica fallbacks ---------------------------
+    def store_update(self, ns, model, variant, accelerator, gpu_count, num_gpu_blocks, block_size, total_kv_tokens, effective):
+        """a live capacity into the store (analyzer.go:184-196), the record's VLLMParams kept"""
+        old = self.store.get(ns, model, variant)
+        self.store.update(ns, model, variant, {"AcceleratorName": accelerator, "GpuCount": gpu_count, "NumGpuBlocks": num_gpu_blocks,
+                                               "BlockSize": block_size, "TotalKvCapacityTokens": total_kv_tokens,
+                                               "EffectiveCapacity": effective, "VLLMParams": old.get("VLLMParams") if old else None,
+                                               "LearnedFrom": "live"})
+
+    def fallback_capacity(self, ns, model, variant, accelerator, gpu_count, kv_thr, avg_in, avg_out) -> float:
+        """the per-replica capacity of a variant without a replica with capacity data (:317-324), read from the store
+        after this cycle's updates; 0.0 = none"""
+        fb, rec = 0.0, self.store.get(ns, model, variant)
+        if rec is not None and rec.get("EffectiveCapacity", 0) > 0:
+            fb = self._stored_capacity(rec, model, kv_thr, avg_in, avg_out)
+        elif rec is not None and rec.get("VLLMParams"):
+            c2 = self.store.find_compatible(model, accelerator, gpu_count, rec["VLLMParams"])
+            if c2 is not None:
+                fb = float(c2.get("EffectiveCapacity", 0))
+        return fb
+
     # -- Analyze ------------------------------------------------------------------------------------------------------
     def analyze(self, inp: dict) -> dict:
         """AnalyzerInput {ModelID, Namespace, ReplicaMetrics, VariantStates, Config, SchedulerQueue} -> AnalyzerResult."""
@@ -508,11 +534,8 @@ class SaturationAnalyzerV2:
             ns, model = inp.get("Namespace", ""), inp.get("ModelID", "")
 
             def update(v, i, eff):
-                old = self.store.get(ns, model, v)
-                self.store.update(ns, model, v, {"AcceleratorName": rms[i].get("AcceleratorName", ""), "GpuCount": gpus.get(v, 0),
-                                                 "NumGpuBlocks": int(rms[i].get("NumGpuBlocks", 0)), "BlockSize": int(rms[i].get("BlockSize", 0)),
-                                                 "TotalKvCapacityTokens": int(rms[i]["TotalKvCapacityTokens"]), "EffectiveCapacity": eff,
-                                                 "VLLMParams": old.get("VLLMParams") if old else None, "LearnedFrom": "live"})
+                self.store_update(ns, model, v, rms[i].get("AcceleratorName", ""), gpus.get(v, 0), int(rms[i].get("NumGpuBlocks", 0)),
+                                  int(rms[i].get("BlockSize", 0)), int(rms[i]["TotalKvCapacityTokens"]), eff)
             for k, v in enumerate(names):
                 vi = mvo[mi] + k
                 if self.device_history:                     # once per slot: its last data replica of the cycle
@@ -533,13 +556,7 @@ class SaturationAnalyzerV2:
                 v = st_["VariantName"]
                 if any(int(rms[i].get("TotalKvCapacityTokens", 0)) > 0 for i in by_var.get(v, [])):
                     continue
-                fb, rec = 0.0, self.store.get(ns, model, v)
-                if rec is not None and rec.get("EffectiveCapacity", 0) > 0:
-                    fb = self._stored_capacity(rec, model, kv_thr, avg_of[0], avg_of[1])
-                elif rec is not None and rec.get("VLLMParams"):
-                    c2 = self.store.find_compatible(model, accel.get(v, ""), int(st_.get("GPUsPerReplica", 0)), rec["VLLMParams"])
-                    if c2 is not None:
-                        fb = float(c2.get("EffectiveCapacity", 0))
+                fb = self.fallback_capacity(ns, model, v, accel.get(v, ""), int(st_.get("GPUsPerReplica", 0)), kv_thr, avg_of[0], avg_of[1])
                 if fb:
                     vfb[mvo[mi] + k] = fb
                     any_fb = True
@@ -604,17 +621,10 @@ class CostAwareOptimizer:
             for k, n in enumerate(names):
                 if n not in st and int(tgt[mvo[mi] + k]) == 0:
                     continue                                   # a capacity without a state only enters targets when it is scaled
-                t, c = int(tgt[mvo[mi] + k]), int(st.get(n, {}).get("CurrentReplicas", 0))
-                if t > c:
-                    action, reason = "scale-up", "V2 scale-up (optimizer: cost-aware, required: %.0f)" % r["Result"].get("RequiredCapacity", 0.0)
-                elif t < c:
-                    action, reason = "scale-down", "V2 scale-down (optimizer: cost-aware, spare: %.0f)" % r["Result"].get("SpareCapacity", 0.0)
-                else:
-                    action, reason = "no-change", "V2 steady state"
                 vc = vc_of.get(n, {})
-                decisions.append({"VariantName": n, "ModelID": r.get("ModelID", ""), "Namespace": r.get("Namespace", ""),
-                                  "AcceleratorName": vc.get("AcceleratorName", ""), "Cost": float(vc.get("Cost", 0.0)),
-                                  "CurrentReplicas": c, "TargetReplicas": t, "Action": action, "Reason": reason})
+                decisions.append(_v2_decision(r.get("ModelID", ""), r.get("Namespace", ""), n, vc.get("AcceleratorName", ""),
+                                              float(vc.get("Cost", 0.0)), int(st.get(n, {}).get("CurrentReplicas", 0)),
+                                              int(tgt[mvo[mi] + k]), r["Result"], self.name()))
         return decisions
 
 
@@ -641,3 +651,96 @@ class Enforcer:
         for i, n in enumerate(names):
             saturation_targets[n] = int(tgt[i])
         return saturation_targets, bool(app[0])
+
+
+# ======================================================================================================================
+# the V2 engine's cycle (optimizeV2, engines/saturation/engine.go:397-488)
+# ======================================================================================================================
+def _v2_decision(model, ns, name, acc, cost, current, target, result, optimizer_name):
+    """CostAwareOptimizer's decision for one variant (cost_aware_optimizer.go), as CostAwareOptimizer.optimize makes it"""
+    if target > current:
+        action, reason = "scale-up", "V2 scale-up (optimizer: %s, required: %.0f)" % (optimizer_name, result.get("RequiredCapacity", 0.0))
+    elif target < current:
+        action, reason = "scale-down", "V2 scale-down (optimizer: %s, spare: %.0f)" % (optimizer_name, result.get("SpareCapacity", 0.0))
+    else:
+        action, reason = "no-change", "V2 steady state"
+    return {"VariantName": name, "ModelID": model, "Namespace": ns, "AcceleratorName": acc, "Cost": cost,
+            "CurrentReplicas": current, "TargetReplicas": target, "Action": action, "Reason": reason}
+
+
+def _apply_enforced(d, enforced, optimizer_name):
+    """applyEnforcedTargetsToDecisions (engine_v2.go:106-127) for one decision"""
+    if enforced != d["TargetReplicas"]:
+        d["TargetReplicas"] = enforced
+        c = d["CurrentReplicas"]
+        d["Action"] = "scale-up" if enforced > c else ("scale-down" if enforced < c else "no-change")
+        d["Reason"] = "V2 %s (optimizer: %s, enforced)" % (d["Action"], optimizer_name)
+
+
+def optimize_v2(analyzer, optimizer, enforcer, inputs, scale_to_zero=None):
+    """optimizeV2 on the host: AnalyzerInputs of the models that make a request -> analyze_batch -> Optimize ->
+    EnforcePolicy per model (extractTargetsFromDecisions / buildVariantAnalysesFromDecisions) -> the enforced targets
+    applied to the decisions.  scale_to_zero: per input, ScaleToZero enabled (default off)."""
+    results = analyzer.analyze_batch(inputs)
+    reqs = [{"ModelID": i.get("ModelID", ""), "Namespace": i.get("Namespace", ""), "Result": r, "VariantStates": i.get("VariantStates", [])}
+            for i, r in zip(inputs, results)]
+    decisions = optimizer.optimize(reqs)
+    of = {}
+    for d in decisions:
+        of.setdefault((d["ModelID"], d["Namespace"]), []).append(d)
+    for k, req in enumerate(reqs):
+        mine = of.get((req["ModelID"], req["Namespace"]), [])
+        targets = {d["VariantName"]: d["TargetReplicas"] for d in mine}
+        analyses = [{"VariantName": d["VariantName"], "AcceleratorName": d["AcceleratorName"], "Cost": d["Cost"],
+                     "ReplicaCount": d["CurrentReplicas"]} for d in mine]
+        enforced, _ = enforcer.enforce_policy(req["ModelID"], req["Namespace"], targets, analyses,
+                                              bool(scale_to_zero[k]) if scale_to_zero is not None else False)
+        for d in mine:
+            if d["VariantName"] in enforced:
+                _apply_enforced(d, enforced[d["VariantName"]], optimizer.name())
+    return decisions
+
+
+def ingest_v2_decisions(ing, analyzer, models, variant_names, accelerator_names, gpus_per_replica, optimizer_name="cost-aware"):
+    """One V2 cycle through an `IngestV2` whose columns the collector has written: analyze() -> the host step on
+    `analyzer`'s capacity store (SaturationAnalyzerV2.store_update once per store slot, then fallback_capacity for the
+    variants without a replica with capacity data: the same code analyze_batch runs) -> decide() -> the VariantDecision
+    dicts optimize_v2 returns, in registry order.  models: [(ModelID, Namespace)] per registry model; variant_names /
+    accelerator_names / gpus_per_replica: per registry variant."""
+    r, c = ing.analyze(), ing.cols
+    mvo = ing.model_variant_off
+    model_of = np.repeat(np.arange(len(mvo) - 1), np.diff(mvo))
+    vslot = ing.var_store_slot
+    last = r["slot_last_rep"][vslot] if len(vslot) else np.zeros(0, np.int32)
+    for v in np.flatnonzero(last >= 0):                    # once per store slot: its last data replica of the cycle
+        v, rep = int(v), int(last[v])
+        pod, (model, ns) = int(r["rep_pod"][rep]), models[model_of[v]]
+        analyzer.store_update(ns, model, variant_names[v], accelerator_names[v], int(gpus_per_replica[v]),
+                              int(c["num_gpu_blocks"][pod]), int(c["block_size"][pod]), int(r["rep_total_kv_tokens"][rep]),
+                              int(r["slot_effective"][vslot[v]]))
+    fb = c["var_fallback_capacity"]
+    fb[:] = 0.0
+    has_req = r["mod_has_request"]
+    for v in np.flatnonzero(r["var_no_data"]):
+        v = int(v)
+        m = int(model_of[v])
+        if not has_req[m]:
+            continue
+        model, ns = models[m]
+        fb[v] = analyzer.fallback_capacity(ns, model, variant_names[v], accelerator_names[v] if r["variant_replica_off"][v + 1] > r["variant_replica_off"][v] else "",
+                                           int(gpus_per_replica[v]), float(c["cfg_kv_threshold"][m]),
+                                           float(r["mod_avg_input_tokens"][m]), float(r["mod_avg_output_tokens"][m]))
+    r = ing.decide()
+    vro = r["variant_replica_off"]
+    out = []
+    for m in np.flatnonzero(has_req):
+        m = int(m)
+        model, ns = models[m]
+        res = {"RequiredCapacity": float(r["mod_required_capacity"][m]), "SpareCapacity": float(r["mod_spare_capacity"][m])}
+        for v in range(int(mvo[m]), int(mvo[m + 1])):
+            rep = vro[v + 1] > vro[v]
+            d = _v2_decision(model, ns, variant_names[v], accelerator_names[v] if rep else "", float(c["var_cost"][v]) if rep else 0.0,
+                             int(c["var_current"][v]), int(r["var_optimizer_target"][v]), res, optimizer_name)
+            _apply_enforced(d, int(r["var_target"][v]), optimizer_name)
+            out.append(d)
+    return out
