@@ -258,6 +258,26 @@ int32_t wva_set_capacity(wva_ctx* ctx, const int32_t* type_count /* [T] */);
 /* System.Calculate (pkg/core/system.go:258-268) -> Server.Calculate (server.go:55-67)
  * -> CreateAllocation (allocation.go:27-155) for every (server, accelerator). */
 int32_t wva_calculate(wva_ctx* ctx);
+/* Replace the per-cycle server columns of the loaded system in place: ServerLoadSpec and CurrentAlloc
+ * (pkg/config/types.go), i.e. what AddServerInfoToSystemData (internal/utils/utils.go:204-240) rewrites every cycle.
+ * All six arrays are [S] and required; srv_cur_acc follows wva_load_system's rule (else WVA_ERR_ARG and nothing
+ * changes).  WVA_ERR_STATE before wva_load_system.  A device pass compares the new values bitwise with the resident
+ * ones (-0.0 vs 0.0 and differing NaN payloads are changes) and marks each server of the ctx's block: re-size when
+ * arrival, in_tokens or out_tokens changed, or cur_acc changed on a keepAccelerator server; re-value when only the
+ * current allocation changed.  Marks accumulate until the next wva_calculate or wva_recalculate.  The candidates are
+ * left as they were; wva_solve, wva_grid_run and wva_analyze_grid read the new columns. */
+int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t* srv_in_tokens,
+                           const int32_t* srv_out_tokens, const int32_t* srv_cur_acc, const int32_t* srv_cur_replicas,
+                           const float* srv_cur_cost);
+/* Bring the candidates up to date with every wva_update_servers since the last wva_calculate / wva_recalculate:
+ * re-size the servers whose sizing inputs changed (the sizer wva_calculate would pick for that many servers, on a
+ * gathered copy of their columns) and re-value the ones whose current allocation alone changed.  The candidates are
+ * bit-equal to those of a wva_calculate, except n_solves, which counts the solves of the sizer that last sized the pair
+ * (the sizers spend different numbers of solves on the same result).  *n_resized / *n_revalued (either may be NULL) get the two counts of the ctx's
+ * block.  WVA_ERR_STATE unless the resident candidates come from wva_calculate / wva_recalculate on the loaded system:
+ * after wva_load_system until the next wva_calculate, after wva_set_candidates, and after a failed sizing.  Timing as
+ * for wva_calculate, with calculate_ms over the whole call; with nothing to re-size sizer_kernel and the counts are 0. */
+int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued);
 /* Manager.Optimize (pkg/manager/manager.go:21-27): Optimizer.Optimize
  * (pkg/solver/optimizer.go:24-36) -> Solver.Solve (solver.go:32-60) — SolveUnlimited
  * (solver.go:63-79) or SolveGreedy (greedy.go:35-105) — then AllocateByType. */

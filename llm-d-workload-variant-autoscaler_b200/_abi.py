@@ -111,6 +111,10 @@ SYSTEM_ARRAYS = {
     "srv_cur_acc": (np.int32, "S"), "srv_cur_replicas": (np.int32, "S"), "srv_cur_cost": (np.float32, "S"),
 }
 
+# the per-cycle server columns wva_update_servers replaces, in its argument order
+CYCLE_ARRAYS = {"srv_arrival": np.float32, "srv_in_tokens": np.int32, "srv_out_tokens": np.int32,
+                "srv_cur_acc": np.int32, "srv_cur_replicas": np.int32, "srv_cur_cost": np.float32}
+
 CAND_ARRAYS = {"state": np.uint8, "num_replicas": np.int32, "batch_size": np.int32, "cost": np.float32,
                "value": np.float32, "itl": np.float32, "ttft": np.float32, "rho": np.float32,
                "max_arrv_rate": np.float32, "n_solves": np.int32}

@@ -19,6 +19,7 @@
 #include "greedy_solve.cuh"
 #include "greedy_sweep.cuh"
 #include "mm1k_kernel.cuh"
+#include "recalc_kernel.cuh"
 #include "ingest_scatter.hpp"
 
 #include <cuda_runtime.h>
@@ -71,7 +72,8 @@ struct PinBuf {  // growable pinned host staging
 // variants / replicas before a group member's block) a column's count is its offset to that block.
 struct Ext { size_t A = 0, T = 0, M = 0, S = 0, V = 0, P = 0, R = 0; };   // P: pairs or replicas, R: grid levels
 enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL too
-       COL_DETAIL = 2 };  // V1 saturation analysis field: written only by a detail run
+       COL_DETAIL = 2,    // V1 saturation analysis field: written only by a detail run
+       COL_CYCLE = 4 };   // server column wva_update_servers replaces in place (ServerLoadSpec and CurrentAlloc)
 
 #define SYS_COLS(X)                                                                                                    \
   X(acc_cost, n.A, 0) X(acc_multiplicity, n.A, 0) X(acc_type, n.A, 0) X(type_count, n.T, 0)                            \
@@ -79,8 +81,9 @@ enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL t
   X(perf_at_tokens, n.M * n.A, 0) X(perf_acc_count, n.M * n.A, 0) X(perf_present, n.M * n.A, 0)                        \
   X(srv_model, n.S, 0) X(srv_priority, n.S, 0) X(srv_min_replicas, n.S, 0) X(srv_max_batch, n.S, 0)                    \
   X(srv_keep_acc, n.S, 0) X(srv_target_present, n.S, 0) X(srv_slo_ttft, n.S, 0) X(srv_slo_itl, n.S, 0)                \
-  X(srv_slo_tps, n.S, 0) X(srv_arrival, n.S, 0) X(srv_in_tokens, n.S, 0) X(srv_out_tokens, n.S, 0)                     \
-  X(srv_cur_acc, n.S, 0) X(srv_cur_replicas, n.S, 0) X(srv_cur_cost, n.S, 0)
+  X(srv_slo_tps, n.S, 0) X(srv_arrival, n.S, COL_CYCLE) X(srv_in_tokens, n.S, COL_CYCLE)                              \
+  X(srv_out_tokens, n.S, COL_CYCLE) X(srv_cur_acc, n.S, COL_CYCLE) X(srv_cur_replicas, n.S, COL_CYCLE)                 \
+  X(srv_cur_cost, n.S, COL_CYCLE)
 #define CAND_COLS(X)                                                                                                   \
   X(state, n.P, 0) X(num_replicas, n.P, 0) X(batch_size, n.P, 0) X(cost, n.P, 0) X(value, n.P, 0) X(itl, n.P, 0)      \
   X(ttft, n.P, 0) X(rho, n.P, 0) X(max_arrv_rate, n.P, 0) X(n_solves, n.P, COL_OPT)
@@ -175,6 +178,25 @@ struct Missing {
   template <class T, class H> void operator()(size_t n, int flags, T*, H* h) { any |= n && !h && !(flags & COL_OPT); }
 };
 
+// visits the per-cycle server columns (COL_CYCLE) of S servers only
+template <class F, class... Structs> static void each_cycle(size_t S, F&& f, Structs&&... s) {
+  Ext n;
+  n.S = S;
+  each_sys(n, [&](size_t c, int flags, auto&&... col) { if (flags & COL_CYCLE) f(c, flags, col...); }, s...);
+}
+
+// The preconditions of the per-cycle columns, shared by wva_load_system and wva_update_servers: every array non-NULL
+// and srv_cur_acc an accelerator index or a WVA_CUR_ACC_* sentinel.  Returns the violated rule, or nullptr.
+static const char* check_cycle_columns(const wva_system& s, size_t S, int A) {
+  Missing miss;
+  SysView none = {};
+  each_cycle(S, miss, none, s);
+  if (miss.any) return "a required array is NULL";
+  for (size_t i = 0; i < S; i++)
+    if (s.srv_cur_acc[i] >= A || s.srv_cur_acc[i] < WVA_CUR_ACC_UNKNOWN) return "srv_cur_acc out of range";
+  return nullptr;
+}
+
 // Sizes an arena with a pass of `lay` over a copy of `f` that has no base, reserves it, then runs `lay` over `f` with the
 // arena as its base.  Nothing is bound and nothing copied unless the reservation succeeds.
 template <class F, class Lay> static cudaError_t lay_out(DevBuf& buf, F& f, Lay&& lay) {
@@ -211,6 +233,8 @@ struct wva_ctx {
 
   // queueing system
   bool loaded = false, calculated = false, solved = false;
+  bool sized = false;               // the resident candidates come from wva_calculate / wva_recalculate on this ctx
+  bool marked = false;              // `marks` holds the marks of a wva_update_servers since then (else all clear)
   bool force_lane_sizer = false;
   int gang_refill = -1;             // lock-step lane sizer: a warp refills only when all its lanes are idle; -1 = by size
   int length_sort = -1;             // lane sizer pulls items through the probe-sorted permutation (sizer_probe.cuh); -1 = by size
@@ -222,6 +246,7 @@ struct wva_ctx {
   uint8_t unlimited = 1, delayed = 0;
   int policy = 0;
   DevBuf sys_arena, cand_arena, sol_arena, scratch, gtab, greedy_ws, split_ws, order_ws, pool_ws;
+  DevBuf marks, cycle_in, recalc_ws, gather_ws;   // wva_update_servers / wva_recalculate
   PinBuf stage_in, stage_out;
   SysView sys = {};
   CandView cand = {};
@@ -319,6 +344,7 @@ int32_t wva_destroy(wva_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   ctx->sys_arena.release(); ctx->cand_arena.release(); ctx->sol_arena.release(); ctx->scratch.release();
+  ctx->marks.release(); ctx->cycle_in.release(); ctx->recalc_ws.release(); ctx->gather_ws.release();
   ctx->gtab.release(); ctx->pool_ws.release(); ctx->greedy_ws.release(); ctx->split_ws.release(); ctx->order_ws.release(); ctx->grid.buf.release(); ctx->grid.defer.release(); ctx->sat.in.release(); ctx->sat.out.release(); ctx->sat.desc.release(); ctx->io_in.release(); ctx->io_out.release();
   ctx->stage_in.release(); ctx->stage_out.release(); ctx->io_stage_in.release(); ctx->io_stage_out.release();
   comm_release(ctx); ctx->comm_ws.release();
@@ -352,10 +378,9 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   // validate indices the kernels dereference (after the NULL checks above)
   for (size_t a = 0; a < A; a++)
     if (s->acc_type[a] < 0 || s->acc_type[a] >= (int)T) { ctx->last_error = "wva_load_system: acc_type out of range"; return WVA_ERR_ARG; }
-  for (size_t i = 0; i < S; i++) {
+  for (size_t i = 0; i < S; i++)
     if (s->srv_model[i] >= (int)M) { ctx->last_error = "wva_load_system: srv_model out of range"; return WVA_ERR_ARG; }
-    if (s->srv_cur_acc[i] >= (int)A || s->srv_cur_acc[i] < WVA_CUR_ACC_UNKNOWN) { ctx->last_error = "wva_load_system: srv_cur_acc out of range"; return WVA_ERR_ARG; }
-  }
+  if (const char* bad = check_cycle_columns(*s, S, (int)A)) { ctx->last_error = std::string("wva_load_system: ") + bad; return WVA_ERR_ARG; }
   // ServiceParms (pkg/analyzer/queueanalyzer.go:33-38) are measured service-time coefficients: finite and >= 0.  A
   // negative or NaN coefficient makes arrival rates negative (QueueModel.Solve's gate, queuemodel.go:31) or NaN and
   // the sizing meaningless; it is rejected here instead of being carried into the kernels.
@@ -400,16 +425,15 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
   ctx->loaded = true; ctx->calculated = false; ctx->solved = false;
+  ctx->sized = false; ctx->marked = false;
   return WVA_OK;
 }
 
 // ------------------------------------------------------------------ calculate
 }  // extern "C" (templates need C++ linkage)
 template <int THREADS, bool SMEM>
-static cudaError_t launch_sizer(wva_ctx* ctx, int blocks, size_t smem, unsigned long long n_pairs, int nmax, float* gtab,
-                                int* ovf_list) {
-  const SysView sys_v = shard_sys(ctx);
-  const CandView cand_v = shard_cand(ctx);
+static cudaError_t launch_sizer(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v, int blocks, size_t smem,
+                                unsigned long long n_pairs, int nmax, float* gtab, int* ovf_list) {
   // lane_sizer_mode 1 = flattened state machine (sizer_kernel.cuh); 2 = lock-step rounds; 3 = lock-step with two
   // chains per lane; 4 = lock-step, every pair split into a TTFT item and an ITL item (mid-size systems); 5 = split
   // items whose second chain evaluates the predicted next bisection point (wva_core.cuh spec2_*)
@@ -476,12 +500,12 @@ static cudaError_t launch_sizer(wva_ctx* ctx, int blocks, size_t smem, unsigned 
   return cudaGetLastError();
 }
 template <int WARPS>
-static cudaError_t launch_sizer_warp(wva_ctx* ctx, int blocks, size_t smem, unsigned long long n_pairs, int nmax,
-                                     int* ovf_list) {
+static cudaError_t launch_sizer_warp(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v, int blocks, size_t smem,
+                                     unsigned long long n_pairs, int nmax, int* ovf_list) {
   auto k = sizer_warp_kernel<WARPS>;
   cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  k<<<blocks, WARPS * 32, smem, ctx->stream>>>(shard_sys(ctx), shard_cand(ctx), n_pairs, nmax, ctx->d_ctr, ovf_list);
+  k<<<blocks, WARPS * 32, smem, ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, ctx->d_ctr, ovf_list);
   ctx->launches++;
   return cudaGetLastError();
 }
@@ -516,14 +540,13 @@ int32_t wva_pool_phases(wva_ctx* ctx, uint64_t* out) {
 }
 #endif
 
-int32_t wva_calculate(wva_ctx* ctx) {
-  if (!ctx) return WVA_ERR_ARG;
-  if (!ctx->loaded) { ctx->last_error = "wva_calculate before wva_load_system"; return WVA_ERR_STATE; }
-  CK(cudaSetDevice(ctx->device));
-  const SysView sys_v = shard_sys(ctx);
-  const CandView cand_v = shard_cand(ctx);
+}  // extern "C"
+
+// CreateAllocation for every (server, accelerator) pair of the view sys_v into the rows of cand_v: the sizer picked by
+// the view's size, then the float64-overflow slow path.  Sets the sizer fields of ctx->timing (calculate_ms: ev[2] to
+// ev[3], the sizer launches).
+static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v) {
   const unsigned long long n_pairs = (unsigned long long)sys_v.n_servers * ctx->A;
-  ctx->shard_status = WVA_ERR_CUDA;   // until this call returns WVA_OK (agreed on by all ranks in wva_solve)
   // scratch: counters + nmax reduction + overflow list.  The split sizer modes process a pair as TWO items and each may
   // append the pair (both chains of an alpha-dominated pair overflow at lambda_max): 2 entries per pair.
   size_t need = 256 + 256 + (size_t)n_pairs * 8 + 1024;
@@ -601,11 +624,11 @@ int32_t wva_calculate(wva_ctx* ctx) {
     if (n_pairs <= (unsigned long long)ctx->sm_count * 32 && warp_tab * 4 + 1024 <= SMEM_PER_SM && !ctx->force_lane_sizer) {
       if (warp_tab * 8 <= 48 * 1024) {
         int per_sm = (int)(SMEM_PER_SM / (warp_tab * 8 + 1024)); if (per_sm > 6) per_sm = 6; if (per_sm < 1) per_sm = 1;
-        e = launch_sizer_warp<8>(ctx, ctx->sm_count * per_sm, warp_tab * 8, n_pairs, nmax, d_ovf);
+        e = launch_sizer_warp<8>(ctx, sys_v, cand_v, ctx->sm_count * per_sm, warp_tab * 8, n_pairs, nmax, d_ovf);
         ctx->timing.sizer_kernel = 1;
       } else {
         int per_sm = (int)(SMEM_PER_SM / (warp_tab * 4 + 1024)); if (per_sm > 8) per_sm = 8; if (per_sm < 1) per_sm = 1;
-        e = launch_sizer_warp<4>(ctx, ctx->sm_count * per_sm, warp_tab * 4, n_pairs, nmax, d_ovf);
+        e = launch_sizer_warp<4>(ctx, sys_v, cand_v, ctx->sm_count * per_sm, warp_tab * 4, n_pairs, nmax, d_ovf);
         ctx->timing.sizer_kernel = 1;
       }
     } else
@@ -617,16 +640,16 @@ int32_t wva_calculate(wva_ctx* ctx) {
       size_t smem = per_lane * best_threads;
       ctx->timing.sizer_kernel = 2;
       switch (best_threads) {
-        case 256: e = launch_sizer<256, true>(ctx, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-        case 192: e = launch_sizer<192, true>(ctx, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-        case 128: e = launch_sizer<128, true>(ctx, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-        default: e = launch_sizer<64, true>(ctx, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+        case 256: e = launch_sizer<256, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+        case 192: e = launch_sizer<192, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+        case 128: e = launch_sizer<128, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+        default: e = launch_sizer<64, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
       }
     } else {
       int blk = ctx->sm_count * 2;
       ctx->timing.sizer_kernel = 3;
       CK(ctx->gtab.reserve((size_t)blk * 256 * per_lane));
-      e = launch_sizer<256, false>(ctx, blk, 0, n_pairs, nmax, (float*)ctx->gtab.p, d_ovf);
+      e = launch_sizer<256, false>(ctx, sys_v, cand_v, blk, 0, n_pairs, nmax, (float*)ctx->gtab.p, d_ovf);
     }
     if (e != cudaSuccess) { ctx->last_error = std::string("sizer launch: ") + cudaGetErrorString(e); return WVA_ERR_CUDA; }
   }
@@ -653,7 +676,166 @@ sizer_done:
     if (rc != 0) { ctx->last_error = "overflow slow path failed"; return WVA_ERR_CUDA; }
     CK(cudaStreamSynchronize(ctx->stream));
   }
+  return WVA_OK;
+}
+
+extern "C" {
+
+int32_t wva_calculate(wva_ctx* ctx) {
+  if (!ctx) return WVA_ERR_ARG;
+  if (!ctx->loaded) { ctx->last_error = "wva_calculate before wva_load_system"; return WVA_ERR_STATE; }
+  CK(cudaSetDevice(ctx->device));
+  ctx->shard_status = WVA_ERR_CUDA;   // until this call returns WVA_OK (agreed on by all ranks in wva_solve)
+  ctx->sized = false;
+  const int32_t rc = size_views(ctx, shard_sys(ctx), shard_cand(ctx));
+  if (rc != WVA_OK) return rc;
   ctx->calculated = true; ctx->solved = false;
+  ctx->sized = true; ctx->marked = false;   // every pair sized from the resident columns: the marks are void
+  ctx->shard_status = WVA_OK;
+  return WVA_OK;
+}
+
+// ------------------------------------------------------------------ per-cycle update
+int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t* srv_in_tokens,
+                           const int32_t* srv_out_tokens, const int32_t* srv_cur_acc, const int32_t* srv_cur_replicas,
+                           const float* srv_cur_cost) {
+  if (!ctx) return WVA_ERR_ARG;
+  if (!ctx->loaded) { ctx->last_error = "wva_update_servers before wva_load_system"; return WVA_ERR_STATE; }
+  wva_system in = {};
+  in.srv_arrival = srv_arrival; in.srv_in_tokens = srv_in_tokens; in.srv_out_tokens = srv_out_tokens;
+  in.srv_cur_acc = srv_cur_acc; in.srv_cur_replicas = srv_cur_replicas; in.srv_cur_cost = srv_cur_cost;
+  const size_t S = (size_t)ctx->S;
+  if (const char* bad = check_cycle_columns(in, S, ctx->A)) { ctx->last_error = std::string("wva_update_servers: ") + bad; return WVA_ERR_ARG; }
+  if (S == 0) return WVA_OK;
+  CK(cudaSetDevice(ctx->device));
+  // the six columns staged at their offsets of one pinned buffer, one H2D copy, then one classify-and-write pass
+  SysView nu = ctx->sys;
+  Layout L;
+  each_cycle(S, L, nu);
+  const size_t total = L.off + 256;
+  CK(ctx->stage_in.reserve(total));
+  CK(ctx->cycle_in.reserve(total));
+  CK(ctx->marks.reserve(S));
+  char* h = (char*)ctx->stage_in.p;
+  L = Layout{(char*)ctx->cycle_in.p};
+  each_cycle(S, [&](size_t c, int, auto*& d, auto* src) { memcpy(h + L.off, src, c * sizeof(*d)); L(c, 0, d); }, nu, in);
+  CK(cudaEventRecord(ctx->ev[0], ctx->stream));
+  CK(cudaMemcpyAsync(ctx->cycle_in.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
+  if (!ctx->marked) CK(cudaMemsetAsync(ctx->marks.p, 0, S, ctx->stream));
+  classify_servers_kernel<<<(unsigned)((S + 255) / 256), 256, 0, ctx->stream>>>(ctx->sys, nu, ctx->shard_lo, ctx->shard_hi,
+                                                                               (unsigned char*)ctx->marks.p);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev[1], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));   // the staging buffer is free for the next call
+  ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
+  ctx->marked = true; ctx->solved = false;
+  return WVA_OK;
+}
+
+}  // extern "C"
+
+// fills `m` with one entry per column the visitor walks: f(count, flags, from, to) moves `from` to `to`
+#define COUNT_COL_(field, count, flags) +1
+static_assert(0 SYS_COLS(COUNT_COL_) <= RowMoves::MAXC && 0 CAND_COLS(COUNT_COL_) <= RowMoves::MAXC,
+              "RowMoves holds every column of either list");
+#undef COUNT_COL_
+struct AddMove {
+  RowMoves& m;
+  template <class T, class U> void operator()(size_t c, int, T* from, U* to) {
+    if (!c) return;
+    m.src[m.n] = (const char*)from; m.dst[m.n] = (char*)to; m.width[m.n] = (int)sizeof(T);
+    m.n++;
+  }
+};
+
+static void launch_move_rows(wva_ctx* ctx, const RowMoves& m, const int* rows, int n_rows, int per, bool scatter) {
+  const unsigned long long n_items = (unsigned long long)n_rows * per;
+  const unsigned long long blocks = std::min<unsigned long long>((n_items + 255) / 256, (unsigned long long)ctx->sm_count * 16);
+  move_rows_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(m, rows, n_items, per, scatter);
+  ctx->launches++;
+}
+
+extern "C" {
+
+int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
+  if (!ctx) return WVA_ERR_ARG;
+  if (n_resized) *n_resized = 0;
+  if (n_revalued) *n_revalued = 0;
+  if (!ctx->loaded) { ctx->last_error = "wva_recalculate before wva_load_system"; return WVA_ERR_STATE; }
+  if (!ctx->sized) {
+    ctx->last_error = "wva_recalculate: the resident candidates do not come from wva_calculate on the loaded system";
+    return WVA_ERR_STATE;
+  }
+  CK(cudaSetDevice(ctx->device));
+  ctx->shard_status = WVA_ERR_CUDA;   // until this call returns WVA_OK (agreed on by all ranks in wva_solve)
+  ctx->sized = false;                 // until every marked server is brought up to date
+  ctx->timing.chain_solves = ctx->timing.chain_states = ctx->timing.overflow_pairs = ctx->timing.certify_fallbacks = 0;
+  ctx->timing.sizer_kernel = 0;
+  const int lo = ctx->shard_lo, n = ctx->shard_hi - ctx->shard_lo, A = ctx->A;
+  CK(cudaEventRecord(ctx->ev[0], ctx->stream));
+  // 1) the rank's marked servers compacted, in server order: the re-size list, then the re-value-only list
+  int cnt[2] = {0, 0};
+  int *resize = nullptr, *revalue = nullptr;
+  if (ctx->marked && n > 0) {
+    const unsigned char* marks = (const unsigned char*)ctx->marks.p;
+    thrust::counting_iterator<int> servers(lo);
+    thrust::discard_iterator<> clean;
+    size_t tmp = 0;
+    CK(cub::DevicePartition::If(nullptr, tmp, servers, (int*)nullptr, (int*)nullptr, clean, (int*)nullptr, n,
+                                MarkedResize{marks}, MarkedRevalueOnly{marks}, ctx->stream));
+    const size_t list = ((size_t)n * 4 + 255) & ~(size_t)255;
+    CK(ctx->recalc_ws.reserve(2 * list + 256 + tmp));
+    resize = (int*)ctx->recalc_ws.p;
+    revalue = (int*)((char*)ctx->recalc_ws.p + list);
+    int* d_cnt = (int*)((char*)ctx->recalc_ws.p + 2 * list);
+    CK(cub::DevicePartition::If((char*)ctx->recalc_ws.p + 2 * list + 256, tmp, servers, resize, revalue, clean, d_cnt, n,
+                                MarkedResize{marks}, MarkedRevalueOnly{marks}, ctx->stream));
+    ctx->launches++;
+    CK(cudaMemsetAsync(ctx->marks.p, 0, ctx->S, ctx->stream));
+    CK(cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  ctx->marked = false;
+  const int D = cnt[0], R = cnt[1];
+  if (D > 0) {
+    // 2) the D servers' columns gathered into a view of D servers (model, perf and accelerator arrays shared) ...
+    Ext g;
+    g.S = (size_t)D; g.P = (size_t)D * A;
+    SysView gsys = ctx->sys;
+    gsys.n_servers = D;
+    CandView gcand = {};
+    Layout G;
+    CK(lay_out(ctx->gather_ws, G, [&](Layout& f) {
+      each_sys(g, [&](size_t c, int fl, auto*& p) { if (c) f(c, fl, p); }, gsys);   // server columns only
+      each_cand(g, f, gcand);
+    }));
+    RowMoves in;
+    each_sys(g, AddMove{in}, ctx->sys, gsys);
+    launch_move_rows(ctx, in, resize, D, 1, false);
+    // 3) ... sized by the dispatch of wva_calculate, picked from D ...
+    const int32_t rc = size_views(ctx, gsys, gcand);
+    if (rc != WVA_OK) return rc;
+    // 4) ... and every candidate field written back over the resident rows
+    RowMoves out;
+    each_cand(g, AddMove{out}, gcand, ctx->cand);
+    launch_move_rows(ctx, out, resize, D, A, true);
+  }
+  // 5) the current allocation alone changed: TransitionPenalty of every candidate again
+  if (R > 0 && A > 0) {
+    const unsigned long long n_items = (unsigned long long)R * A;
+    const unsigned long long blocks = std::min<unsigned long long>((n_items + 255) / 256, (unsigned long long)ctx->sm_count * 16);
+    revalue_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(ctx->sys, ctx->cand, revalue, n_items);
+    ctx->launches++;
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev[3], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->timing.calculate_ms = elapsed(ctx, 0, 3);
+  if (n_resized) *n_resized = D;
+  if (n_revalued) *n_revalued = R;
+  ctx->calculated = true; ctx->solved = false;
+  ctx->sized = true;
   ctx->shard_status = WVA_OK;
   return WVA_OK;
 }
@@ -773,6 +955,7 @@ int32_t wva_set_candidates(wva_ctx* ctx, const wva_candidates* in) {
   CK(cudaStreamSynchronize(ctx->stream));               // the caller's buffers are free again on return (cgo pointer rule)
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
   ctx->calculated = true; ctx->solved = false;
+  ctx->sized = false;   // the caller's candidates: wva_recalculate cannot bring them up to date
   return WVA_OK;
 }
 

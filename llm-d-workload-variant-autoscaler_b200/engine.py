@@ -5,6 +5,8 @@ entry points they replace:
 
     load_system      System.SetFromSpec           pkg/core/system.go:82
     calculate        System.Calculate             pkg/core/system.go:258
+    update_servers   AddServerInfoToSystemData    internal/utils/utils.go:204 (loads + current allocations)
+    recalculate      System.Calculate, for the servers update_servers changed
     solve            Manager.Optimize             pkg/manager/manager.go:21
     candidates       Server.AllAllocations        pkg/core/server.go:138
     solution         System.GenerateSolution      pkg/core/system.go:303
@@ -90,6 +92,8 @@ def load_library():
     L.wva_ingest_v2_decide.argtypes = [ctxp]
     L.wva_load_system.argtypes = [ctxp, C.POINTER(abi.System)]
     L.wva_calculate.argtypes = [ctxp]
+    L.wva_update_servers.argtypes = [ctxp] + [C.c_void_p] * len(abi.CYCLE_ARRAYS)
+    L.wva_recalculate.argtypes = [ctxp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.wva_solve.argtypes = [ctxp]
     L.wva_get_candidates.argtypes = [ctxp, C.POINTER(abi.Candidates)]
     L.wva_set_candidates.argtypes = [ctxp, C.POINTER(abi.Candidates)]
@@ -123,7 +127,7 @@ def load_library():
 
 
 EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_last_error", "wva_launch_count",
-           "wva_load_system", "wva_calculate", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
+           "wva_load_system", "wva_calculate", "wva_update_servers", "wva_recalculate", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
            "wva_analyze_grid", "wva_grid_run", "wva_grid_fetch", "wva_mm1k_eval", "wva_saturation_v1",
            "wva_saturation_upload", "wva_saturation_run", "wva_saturation_fetch", "wva_limit", "wva_saturation_v2",
            "wva_cost_aware_optimize", "wva_enforce", "wva_pipeline_v2", "wva_host_alloc", "wva_host_free", "wva_last_timing",
@@ -241,6 +245,24 @@ class Engine:
 
     def calculate(self):
         self._check(self.lib.wva_calculate(self.ctx), "wva_calculate")
+
+    def update_servers(self, arrival, in_tokens, out_tokens, cur_acc, cur_replicas, cur_cost):
+        """The per-cycle server columns of the loaded system (ServerLoadSpec, CurrentAlloc), replaced in place; [S]
+        arrays.  The servers they change are re-sized or re-valued by the next recalculate()."""
+        cols = []
+        for (name, dt), a in zip(abi.CYCLE_ARRAYS.items(), (arrival, in_tokens, out_tokens, cur_acc, cur_replicas, cur_cost)):
+            a = np.ascontiguousarray(a, dt).reshape(-1)
+            if a.size != self.S:
+                raise WvaError(f"update_servers: {name} has {a.size} elements, the loaded system has {self.S} servers")
+            cols.append(a if a.size else np.zeros(1, dt))
+        self._check(self.lib.wva_update_servers(self.ctx, *[a.ctypes.data for a in cols]), "wva_update_servers")
+
+    def recalculate(self):
+        """Candidates brought up to date with the update_servers calls since the last calculate / recalculate, equal to a
+        calculate().  Returns (servers re-sized, servers re-valued) of this context's block."""
+        nr, nv = C.c_int64(), C.c_int64()
+        self._check(self.lib.wva_recalculate(self.ctx, C.byref(nr), C.byref(nv)), "wva_recalculate")
+        return nr.value, nv.value
 
     def solve(self):
         self._check(self.lib.wva_solve(self.ctx), "wva_solve")

@@ -70,6 +70,39 @@ func (x *Ctx) err(rc C.int32_t, what string) error {
 	return fmt.Errorf("%s: %s %s", what, C.GoString(C.wva_strerror(rc)), C.GoString(C.wva_last_error(x.c)))
 }
 
+// UpdateServers replaces the per-cycle server columns of the loaded system (ServerLoadSpec and CurrentAlloc, in the
+// server index order of the loaded system; all [S]) in place; Recalculate then re-sizes or re-values only the servers
+// they changed, with the candidates of a full wva_calculate (INTEGRATION.md §3, per-cycle use).
+func (x *Ctx) UpdateServers(arrival []float32, inTokens, outTokens, curAcc, curReplicas []int32, curCost []float32) error {
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	n := len(arrival)
+	if len(inTokens) != n || len(outTokens) != n || len(curAcc) != n || len(curReplicas) != n || len(curCost) != n {
+		return fmt.Errorf("UpdateServers: the six columns differ in length")
+	}
+	if n == 0 {
+		return x.err(C.wva_update_servers(x.c, nil, nil, nil, nil, nil, nil), "wva_update_servers")
+	}
+	var pin runtime.Pinner // C copies the columns before returning
+	defer pin.Unpin()
+	for _, p := range []unsafe.Pointer{unsafe.Pointer(&arrival[0]), unsafe.Pointer(&inTokens[0]), unsafe.Pointer(&outTokens[0]),
+		unsafe.Pointer(&curAcc[0]), unsafe.Pointer(&curReplicas[0]), unsafe.Pointer(&curCost[0])} {
+		pin.Pin(p)
+	}
+	return x.err(C.wva_update_servers(x.c, (*C.float)(unsafe.Pointer(&arrival[0])), (*C.int32_t)(unsafe.Pointer(&inTokens[0])),
+		(*C.int32_t)(unsafe.Pointer(&outTokens[0])), (*C.int32_t)(unsafe.Pointer(&curAcc[0])),
+		(*C.int32_t)(unsafe.Pointer(&curReplicas[0])), (*C.float)(unsafe.Pointer(&curCost[0]))), "wva_update_servers")
+}
+
+// Recalculate returns how many servers of this context's block were re-sized and re-valued.
+func (x *Ctx) Recalculate() (resized, revalued int64, err error) {
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	var r, v C.int64_t
+	err = x.err(C.wva_recalculate(x.c, &r, &v), "wva_recalculate")
+	return int64(r), int64(v), err
+}
+
 // index maps built from SORTED names: ascending index is then a valid Go map order and the
 // name-based tie-breaks of the reference become index comparisons.
 type index struct {

@@ -12,6 +12,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from ._abi import CYCLE_ARRAYS
+
 # pkg/config/defaults.go:24-33
 DEFAULT_SERVICE_CLASS_NAME = "Free"
 DEFAULT_LOW_PRIORITY = 100
@@ -131,6 +133,24 @@ def flatten_spec(spec: dict):
     return d, idx
 
 
+def differs_only_in_cycle_columns(old: dict, new: dict) -> bool:
+    """True when two flattened specs describe the same system up to the per-cycle server columns (loads and current
+    allocations, CYCLE_ARRAYS): every other array equal byte for byte, every scalar equal."""
+    if old.keys() != new.keys():
+        return False
+    for k, a in old.items():
+        if k in CYCLE_ARRAYS:
+            continue
+        b = new[k]
+        if isinstance(a, np.ndarray) or isinstance(b, np.ndarray):
+            a, b = np.asarray(a), np.asarray(b)
+            if a.dtype != b.dtype or a.shape != b.shape or a.tobytes() != b.tobytes():
+                return False
+        elif a != b:
+            return False
+    return True
+
+
 def solution_to_spec(sol: dict, idx: SpecIndex, spec_servers: dict | None = None) -> dict:
     """Solution arrays -> config.AllocationSolution JSON shape (System.GenerateSolution, system.go:303-330):
     a server with no allocation is absent; the zero-load allocation has accelerator ""."""
@@ -156,10 +176,37 @@ class Manager:
         self.engine = engine
         self.spec = spec["system"] if "system" in spec and "acceleratorData" not in spec else spec
         self.sysd, self.index = flatten_spec(self.spec)
+        self._sized = False        # the engine holds self.sysd and its candidates from calculate / recalculate
 
     def optimize(self) -> dict:
         """Returns the AllocationSolution (JSON shape).  Raises WvaError where the reference returns an error."""
+        self._sized = False
         sol = self.engine.optimize(self.sysd)
+        self._sized = True
+        return self._solution(sol)
+
+    def update(self, spec: dict) -> dict:
+        """One reconcile cycle on a rebuilt SystemSpec, the same result as `Manager(engine, spec).optimize()`.  When the
+        new spec differs from the one on the device only in server loads and current allocations, those columns are
+        replaced in place and only the servers they changed are re-sized or re-valued (update_servers -> recalculate
+        -> solve); any other change reloads the system (load_system -> calculate -> solve)."""
+        spec = spec["system"] if "system" in spec and "acceleratorData" not in spec else spec
+        sysd, index = flatten_spec(spec)
+        incremental = self._sized and differs_only_in_cycle_columns(self.sysd, sysd)
+        self.spec, self.sysd, self.index, self._cand = spec, sysd, index, None
+        self._sized = False
+        eng = self.engine
+        if incremental:
+            eng.update_servers(*(sysd[k] for k in CYCLE_ARRAYS))
+            eng.recalculate()
+        else:
+            eng.load_system(sysd)
+            eng.calculate()
+        self._sized = True
+        eng.solve()
+        return self._solution(eng.solution())
+
+    def _solution(self, sol: dict) -> dict:
         self.last_solution = sol
         servers = {s["name"]: s for s in _get(self.spec, "serverData", "servers", default=[]) or []}
         return solution_to_spec(sol, self.index, servers)
@@ -173,8 +220,10 @@ class Manager:
         if i is None:
             return {"Allocations": {}}
         if getattr(self, "_cand", None) is None:
+            self._sized = False
             self.engine.load_system(self.sysd)
             self.engine.calculate()
+            self._sized = True
             self._cand = self.engine.candidates()
         c = self._cand
         out = {}
