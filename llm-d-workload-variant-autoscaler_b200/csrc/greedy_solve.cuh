@@ -77,7 +77,7 @@ struct GreedyWs {   // device workspace views
   // bestEffort filter: the capacity types (< 64) behind a server's candidates, and per type the smallest units per replica
   // of any candidate — a server none of whose types has that much left can get nothing (greedy.go:204-213, 262-272)
   g_u64* tmask; long long* min_upr;
-  long long* stats;  // [2] heap pushes, events (entries processed) of the last sweep
+  long long* stats;  // heap pushes, events (entries processed), largest heap of the last sweep (the event sweep: [25])
 };
 
 __global__ void __launch_bounds__(128) greedy_prepare_kernel(SysView s, CandView c, GreedyWs w) {
@@ -486,6 +486,7 @@ __global__ void __launch_bounds__(32, 1) greedy_allocate_kernel(SysView s, Greed
   unsigned tau = 0;
   long long n_events = 0;
   int head = 0, n_un = 0, group_un0 = 0, base = -32;
+  int heap_max = 0;                                 // most entries the heap held at once (past G_HEAP_SM: the global tier)
   g_u64 l_khi = 0; unsigned l_kv = 0; int l_type = -1, l_srv = -1; long long l_cnt = 0;   // this lane's head record
   unsigned group_pw = 0;
   bool group_set = false, batch_staged = false;
@@ -640,11 +641,12 @@ __global__ void __launch_bounds__(32, 1) greedy_allocate_kernel(SysView s, Greed
     ne.khi = stop_khi; ne.klo = ((g_u64)stop_kv << 32) | (unsigned)~(++tau);
     ne.cnt = stop_cnt; ne.srv = srv; ne.ci = stop_j; ne.type = stop_type;
     { GP_T(t_push); heap.push(ne); GP_ADD(4, t_push); GP_INC(11); }
+    if (heap.n > heap_max) heap_max = heap.n;
   }
   __syncwarp();
   { GP_T(t_be); if (delayed) g_best_effort(s, w, avail, w.unalloc, n_un, policy); GP_ADD(6, t_be); }
   GP_ADD(7, t_all);
-  if (writer) { w.stats[0] = (long long)tau; w.stats[1] = n_events; }
+  if (writer) { w.stats[0] = (long long)tau; w.stats[1] = n_events; w.stats[2] = heap_max; }
 #ifdef WVA_GREEDY_PROFILE
   if (writer) for (int i = 0; i < 16; i++) g_prof[i] = prof[i];
 #endif
@@ -768,8 +770,12 @@ static inline int32_t run_solve_greedy(const SysView& s, const CandView& c, cons
   greedy_finalize_kernel<<<nb, 256, 0, stream>>>(s, c, o, w);
   *launches += 2;
   if (stats_out) {
-    if (cudaMemcpyAsync(stats_out, w.stats, 16, cudaMemcpyDeviceToHost, stream) != cudaSuccess) return WVA_ERR_CUDA;
+    long long h[3];
+    if (cudaMemcpyAsync(h, w.stats, sizeof(h), cudaMemcpyDeviceToHost, stream) != cudaSuccess) return WVA_ERR_CUDA;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return WVA_ERR_CUDA;
+    stats_out[0] = h[0]; stats_out[1] = h[1];
+    if (getenv("WVA_SIZER_DEBUG"))
+      fprintf(stderr, "greedy queue: heap pushes %lld, events %lld, largest heap %lld (%d slots in shared memory)\n", h[0], h[1], h[2], G_HEAP_SM);
   }
 #ifdef WVA_GREEDY_PROFILE
   {

@@ -239,6 +239,7 @@ __device__ __forceinline__ int gsw_tie_group(const GreedyWs& w, const GSweepWs& 
     if (nin < 32) break;
   }
   const int end_pos = i;
+  z.d_nact += n_act; if (n_act > z.d_maxact) z.d_maxact = n_act;
   if (n_act <= 1) return -1;
   __syncwarp();
   __threadfence_block();
@@ -414,6 +415,7 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
   GSweepState z = {0, 0, 0, 0, 0, 0, 0};
   int group_un0 = 0;
   long long n_batches = 0, n_rounds = 0, n_seq = 0, n_tie = 0, cyc_be = 0, cyc_tie = 0, n_unalloc_be = 0;
+  long long n_tie_global = 0, n_restart = 0;   // tie groups ordered in global memory; event streams restarted after a jump
   const long long cyc0 = GSW_CLK();
 
   // event stream: blocks of GSW_BLOCK records copied asynchronously into a ring of GSW_SLOTS slots; while block b is
@@ -655,7 +657,7 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
           n_tie++;
           const long long c0 = GSW_CLK();
           int np = gsw_tie_group_staged(w, g, avail, alive, z, pos + first, n_ev, tie_ev, tie_dyn);
-          if (np == -2) np = gsw_tie_group(w, g, avail, alive, z, pos + first, n_ev);
+          if (np == -2) { n_tie_global++; np = gsw_tie_group(w, g, avail, alive, z, pos + first, n_ev); }
           cyc_tie += GSW_CLK() - c0;
           if (np >= 0) { jump = np; break; }
         }
@@ -670,6 +672,7 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
         gsw_wait<0>();
         __syncwarp();
         origin = pos; issued = 0; cur_block = -1;
+        n_restart++;
       }
     } else {
       pos += nvalid;
@@ -683,7 +686,7 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
     g_best_effort(s, w, avail, w.unalloc + group_un0, z.n_un - group_un0, policy, be_stage);
     cyc_be += GSW_CLK() - c0; n_unalloc_be += z.n_un - group_un0;
   }
-  if (lane == 0) { w.stats[8] = cyc_be; w.stats[9] = cyc_tie; w.stats[10] = GSW_CLK() - cyc0; w.stats[11] = n_unalloc_be; w.stats[12] = z.d_fb; w.stats[13] = z.d_nact; w.stats[14] = z.d_maxact; w.stats[15] = z.d_fbev; w.stats[16] = cyc_chk; w.stats[17] = cyc_ring; w.stats[18] = cyc_dead; w.stats[19] = cyc_fast; w.stats[20] = cyc_slow; w.stats[21] = n_survivors; w.stats[23] = n_skip128; }
+  if (lane == 0) { w.stats[8] = cyc_be; w.stats[9] = cyc_tie; w.stats[10] = GSW_CLK() - cyc0; w.stats[11] = n_unalloc_be; w.stats[12] = z.d_fb; w.stats[13] = z.d_nact; w.stats[14] = z.d_maxact; w.stats[15] = z.d_fbev; w.stats[16] = cyc_chk; w.stats[17] = cyc_ring; w.stats[18] = cyc_dead; w.stats[19] = cyc_fast; w.stats[20] = cyc_slow; w.stats[21] = n_survivors; w.stats[22] = n_tie_global; w.stats[23] = n_skip128; w.stats[24] = n_restart; }
   if (lane == 0) { w.stats[0] = 0; w.stats[1] = z.n_active; w.stats[2] = n_batches; w.stats[3] = n_rounds; w.stats[4] = n_seq; w.stats[5] = n_tie; w.stats[6] = pos; w.stats[7] = n_ev; }
 }
 
@@ -758,8 +761,8 @@ static inline int32_t run_solve_greedy_sweep(const SysView& s, const CandView& c
     if (cudaStreamSynchronize(stream) != cudaSuccess) return WVA_ERR_CUDA;
     stats_out[0] = h[0]; stats_out[1] = h[1];
     if (getenv("WVA_SIZER_DEBUG"))
-      fprintf(stderr, "greedy sweep: alive events %lld, batches %lld, rounds %lld, sequential events %lld, tie-group calls %lld, stopped at %lld of %lld; cycles: best effort %lld (%lld entries), tie groups %lld, kernel %lld; tie groups: %lld over the staging size (%lld events), alive leaders %lld (max %lld); loop cycles: early-exit check %lld, ring %lld, dead batches %lld, fast path %lld, slow path %lld; entries swept on after nothing fits: %lld; 128-event skips %lld\n",
-              h[1], h[2], h[3], h[4], h[5], h[6], h[7], h[8], h[11], h[9], h[10], h[12], h[15], h[13], h[14], h[16], h[17], h[18], h[19], h[20], h[21], h[23]);
+      fprintf(stderr, "greedy sweep: alive events %lld, batches %lld, rounds %lld, sequential events %lld, tie-group calls %lld, stopped at %lld of %lld; cycles: best effort %lld (%lld entries), tie groups %lld, kernel %lld; tie groups: %lld over the staging size (%lld events), %lld in global memory, alive leaders %lld (max %lld); loop cycles: early-exit check %lld, ring %lld, dead batches %lld, fast path %lld, slow path %lld; entries swept on after nothing fits: %lld; 128-event skips %lld; stream restarts %lld\n",
+              h[1], h[2], h[3], h[4], h[5], h[6], h[7], h[8], h[11], h[9], h[10], h[12], h[15], h[22], h[13], h[14], h[16], h[17], h[18], h[19], h[20], h[21], h[23], h[24]);
   }
   return cudaGetLastError() == cudaSuccess ? WVA_OK : WVA_ERR_CUDA;
 }
