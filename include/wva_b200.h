@@ -264,8 +264,9 @@ int32_t wva_calculate(wva_ctx* ctx);
  * changes).  WVA_ERR_STATE before wva_load_system.  A device pass compares the new values bitwise with the resident
  * ones (-0.0 vs 0.0 and differing NaN payloads are changes) and marks each server of the ctx's block: re-size when
  * arrival, in_tokens or out_tokens changed, or cur_acc changed on a keepAccelerator server; re-value when only the
- * current allocation changed.  Marks accumulate until the next wva_calculate or wva_recalculate.  The candidates are
- * left as they were; wva_solve, wva_grid_run and wva_analyze_grid read the new columns. */
+ * current allocation changed.  Marks accumulate until the next wva_calculate or wva_recalculate.  The servers whose
+ * load changed also get a grid mark, which accumulates until the next wva_grid_run or wva_grid_update.  The candidates
+ * and the resident grid are left as they were; wva_solve, wva_grid_run and wva_analyze_grid read the new columns. */
 int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t* srv_in_tokens,
                            const int32_t* srv_out_tokens, const int32_t* srv_cur_acc, const int32_t* srv_cur_replicas,
                            const float* srv_cur_cost);
@@ -318,6 +319,19 @@ int32_t wva_analyze_grid(wva_ctx* ctx, int32_t R, uint8_t* ok, float* ttft,
 int32_t wva_grid_run(wva_ctx* ctx, int32_t R, int32_t full);
 int32_t wva_grid_fetch(wva_ctx* ctx, uint8_t* ok, float* ttft, float* itl,
                        float* rho, float* tput, int32_t* frontier);
+/* Bring the resident grid of the last wva_grid_run up to date with every wva_update_servers since the last
+ * wva_grid_run / wva_grid_update: re-evaluate, at the same R and with the same outputs (full or frontier only), the
+ * servers of the ctx's block whose arrival, in_tokens or out_tokens changed (bitwise), and write their rows over the
+ * resident ones (in place when every server of the block changed).  *n_regridded (may be NULL) = that number of
+ * servers.  The grid is bit-equal to that of a
+ * wva_grid_run on the updated system: a server's rows read no current-allocation column.  These grid marks are apart
+ * from the sizing marks: wva_calculate / wva_recalculate leave them, and the grid calls leave the sizing marks.  The
+ * deferred pass and the batch size limit are decided from the re-evaluated servers; the float64-overflow list has the
+ * capacity of a run on the whole block.  WVA_ERR_STATE unless the resident grid comes from wva_grid_run /
+ * wva_grid_update on the loaded system: before wva_load_system, after it until the next wva_grid_run, and after a
+ * failed grid call.  grid_ms covers the whole call; chain_solves, chain_states, overflow_pairs and certify_fallbacks
+ * are those of the re-evaluated servers, 0 when none. */
+int32_t wva_grid_update(wva_ctx* ctx, int64_t* n_regridded);
 
 /*
  * Closed-form M/M/1/K leg: MM1KModel.Solve (pkg/analyzer/mm1kmodel.go:30-92).

@@ -210,9 +210,12 @@ template <class F, class Lay> static cudaError_t lay_out(DevBuf& buf, F& f, Lay&
 struct GridState {   // results of the last wva_grid_run, resident in HBM
   int R = 0;
   bool full = false, ran = false;
+  bool current = false;        // the resident grid comes from wva_grid_run / wva_grid_update on the loaded system
   DevBuf buf, defer;
   GridOut view = {};
   GridCounters* ctr = nullptr;
+  int* nmax = nullptr;         // device word of the max batch pass
+  GridOverflowList ovf = {};   // the block's float64-overflow list, also used by wva_grid_update
 };
 struct SatState {    // resident inputs / outputs of the saturation model
   bool uploaded = false, ran = false;
@@ -235,6 +238,7 @@ struct wva_ctx {
   bool loaded = false, calculated = false, solved = false;
   bool sized = false;               // the resident candidates come from wva_calculate / wva_recalculate on this ctx
   bool marked = false;              // `marks` holds the marks of a wva_update_servers since then (else all clear)
+  bool grid_marked = false;         // `grid_marks` holds the load changes since the last wva_grid_run / wva_grid_update
   bool force_lane_sizer = false;
   int gang_refill = -1;             // lock-step lane sizer: a warp refills only when all its lanes are idle; -1 = by size
   int length_sort = -1;             // lane sizer pulls items through the probe-sorted permutation (sizer_probe.cuh); -1 = by size
@@ -246,7 +250,7 @@ struct wva_ctx {
   uint8_t unlimited = 1, delayed = 0;
   int policy = 0;
   DevBuf sys_arena, cand_arena, sol_arena, scratch, gtab, greedy_ws, split_ws, order_ws, pool_ws;
-  DevBuf marks, cycle_in, recalc_ws, gather_ws;   // wva_update_servers / wva_recalculate
+  DevBuf marks, grid_marks, cycle_in, recalc_ws, gather_ws;   // wva_update_servers / wva_recalculate / wva_grid_update
   PinBuf stage_in, stage_out;
   SysView sys = {};
   CandView cand = {};
@@ -344,7 +348,7 @@ int32_t wva_destroy(wva_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   ctx->sys_arena.release(); ctx->cand_arena.release(); ctx->sol_arena.release(); ctx->scratch.release();
-  ctx->marks.release(); ctx->cycle_in.release(); ctx->recalc_ws.release(); ctx->gather_ws.release();
+  ctx->marks.release(); ctx->grid_marks.release(); ctx->cycle_in.release(); ctx->recalc_ws.release(); ctx->gather_ws.release();
   ctx->gtab.release(); ctx->pool_ws.release(); ctx->greedy_ws.release(); ctx->split_ws.release(); ctx->order_ws.release(); ctx->grid.buf.release(); ctx->grid.defer.release(); ctx->sat.in.release(); ctx->sat.out.release(); ctx->sat.desc.release(); ctx->io_in.release(); ctx->io_out.release();
   ctx->stage_in.release(); ctx->stage_out.release(); ctx->io_stage_in.release(); ctx->io_stage_out.release();
   comm_release(ctx); ctx->comm_ws.release();
@@ -426,6 +430,7 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
   ctx->loaded = true; ctx->calculated = false; ctx->solved = false;
   ctx->sized = false; ctx->marked = false;
+  ctx->grid.current = false; ctx->grid_marked = false;
   return WVA_OK;
 }
 
@@ -716,20 +721,23 @@ int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t
   CK(ctx->stage_in.reserve(total));
   CK(ctx->cycle_in.reserve(total));
   CK(ctx->marks.reserve(S));
+  CK(ctx->grid_marks.reserve(S));
   char* h = (char*)ctx->stage_in.p;
   L = Layout{(char*)ctx->cycle_in.p};
   each_cycle(S, [&](size_t c, int, auto*& d, auto* src) { memcpy(h + L.off, src, c * sizeof(*d)); L(c, 0, d); }, nu, in);
   CK(cudaEventRecord(ctx->ev[0], ctx->stream));
   CK(cudaMemcpyAsync(ctx->cycle_in.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
   if (!ctx->marked) CK(cudaMemsetAsync(ctx->marks.p, 0, S, ctx->stream));
+  if (!ctx->grid_marked) CK(cudaMemsetAsync(ctx->grid_marks.p, 0, S, ctx->stream));
   classify_servers_kernel<<<(unsigned)((S + 255) / 256), 256, 0, ctx->stream>>>(ctx->sys, nu, ctx->shard_lo, ctx->shard_hi,
-                                                                               (unsigned char*)ctx->marks.p);
+                                                                               (unsigned char*)ctx->marks.p,
+                                                                               (unsigned char*)ctx->grid_marks.p);
   ctx->launches++;
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));   // the staging buffer is free for the next call
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
-  ctx->marked = true; ctx->solved = false;
+  ctx->marked = true; ctx->grid_marked = true; ctx->solved = false;
   return WVA_OK;
 }
 

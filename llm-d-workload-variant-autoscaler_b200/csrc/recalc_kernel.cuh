@@ -1,7 +1,7 @@
 // recalc_kernel.cuh — device side of wva_update_servers / wva_recalculate: the per-cycle server columns (load and
 // current allocation) compared with the resident ones and written over them, and the row moves and re-valuation
 // around a sizer run on the servers whose sizing inputs changed.  The sizers themselves are the ones wva_calculate
-// runs, handed a gathered view.
+// runs, handed a gathered view; wva_grid_update moves grid rows around a grid run on a gathered view the same way.
 #pragma once
 #include "wva_core.cuh"
 #include <cuda_runtime.h>
@@ -19,7 +19,10 @@ __device__ __forceinline__ bool bits_differ(float a, float b) { return __float_a
 
 // One pass over the S servers: the bitwise diff of the six per-cycle columns of `nu` against the resident `res`, the
 // write of `nu` over `res`, and the marks of the servers in [lo, hi) (the rank's block; every rank holds every column).
-__global__ void classify_servers_kernel(SysView res, SysView nu, int lo, int hi, unsigned char* marks) {
+// grid_marks[srv] = 1 when the load changed: a server's grid rows read no other per-cycle column (grid_setup), and they
+// accumulate until the next wva_grid_run / wva_grid_update, apart from the sizing marks.
+__global__ void classify_servers_kernel(SysView res, SysView nu, int lo, int hi, unsigned char* marks,
+                                        unsigned char* grid_marks) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= res.n_servers) return;
   const float arr = nu.srv_arrival[i], cost = nu.srv_cur_cost[i];
@@ -38,6 +41,7 @@ __global__ void classify_servers_kernel(SysView res, SysView nu, int lo, int hi,
   const_cast<int*>(res.srv_cur_replicas)[i] = rep;
   const_cast<float*>(res.srv_cur_cost)[i] = cost;
   if (i >= lo && i < hi && (resize || alloc)) marks[i] |= (resize ? MARK_RESIZE : 0) | (alloc ? MARK_REVALUE : 0);
+  if (i >= lo && i < hi && load) grid_marks[i] = 1;
 }
 
 // the two lists wva_recalculate compacts from the marks (a re-sized server is re-valued by its sizing already)

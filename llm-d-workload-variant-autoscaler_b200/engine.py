@@ -11,6 +11,7 @@ entry points they replace:
     candidates       Server.AllAllocations        pkg/core/server.go:138
     solution         System.GenerateSolution      pkg/core/system.go:303
     analyze_grid     QueueAnalyzer.Analyze grid   pkg/analyzer/queueanalyzer.go:127
+    grid_update      the resident grid, for the servers whose load update_servers changed
     mm1k_eval        MM1KModel.Solve              pkg/analyzer/mm1kmodel.go:30
     saturation_v1    AnalyzeModelSaturation + CalculateSaturationTargets
                                                   internal/saturation/analyzer.go:31,290
@@ -101,6 +102,7 @@ def load_library():
     L.wva_analyze_grid.argtypes = [ctxp, C.c_int32] + [C.c_void_p] * 6
     L.wva_grid_run.argtypes = [ctxp, C.c_int32, C.c_int32]
     L.wva_grid_fetch.argtypes = [ctxp] + [C.c_void_p] * 6
+    L.wva_grid_update.argtypes = [ctxp, C.POINTER(C.c_int64)]
     L.wva_saturation_upload.argtypes = [ctxp, C.POINTER(abi.SaturationIn)]
     L.wva_saturation_run.argtypes = [ctxp, C.c_int32]
     L.wva_saturation_fetch.argtypes = [ctxp, C.POINTER(abi.SaturationOut)]
@@ -128,7 +130,7 @@ def load_library():
 
 EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_last_error", "wva_launch_count",
            "wva_load_system", "wva_calculate", "wva_update_servers", "wva_recalculate", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
-           "wva_analyze_grid", "wva_grid_run", "wva_grid_fetch", "wva_mm1k_eval", "wva_saturation_v1",
+           "wva_analyze_grid", "wva_grid_run", "wva_grid_fetch", "wva_grid_update", "wva_mm1k_eval", "wva_saturation_v1",
            "wva_saturation_upload", "wva_saturation_run", "wva_saturation_fetch", "wva_limit", "wva_saturation_v2",
            "wva_cost_aware_optimize", "wva_enforce", "wva_pipeline_v2", "wva_host_alloc", "wva_host_free", "wva_last_timing",
            "wva_microbench_fp64", "wva_set_optimizer", "wva_set_capacity", "wva_comm_unique_id", "wva_comm_init_rank",
@@ -191,6 +193,7 @@ class Engine:
         self.S = self.A = self.T = 0
         self.lo = self.hi = 0          # block of servers this context sizes (the whole system without a communicator)
         self.world, self.rank = 1, 0
+        self._grid_R = 0               # R of the resident grid (grid_run / analyze_grid)
         # optional allocator (name, n, dtype) -> 1-D array for the result buffers of saturation_fetch() and limit(),
         # e.g. views of page-locked buffers from pinned_empty() that the caller reuses from batch to batch
         self.host_alloc = None
@@ -305,6 +308,7 @@ class Engine:
         p = lambda k: out[k].ctypes.data if k in out else None
         self._check(self.lib.wva_analyze_grid(self.ctx, R, p("ok"), p("ttft"), p("itl"), p("rho"), p("tput"),
                                               p("frontier")), "wva_analyze_grid")
+        self._grid_R = R
         for k in list(out):
             out[k] = out[k][: S * A].reshape(S, A) if k == "frontier" else out[k][:n].reshape(S, A, R)
         return out
@@ -312,6 +316,32 @@ class Engine:
     def grid_run(self, R: int, full: bool = False):
         """Grid on the resident system, results stay in HBM (bench: device-resident timing)."""
         self._check(self.lib.wva_grid_run(self.ctx, R, 1 if full else 0), "wva_grid_run")
+        self._grid_R = R
+
+    def grid_update(self):
+        """The resident grid brought up to date with the update_servers calls since the last grid_run / grid_update,
+        equal to a grid_run.  Returns the number of servers of this context's block re-evaluated (load changed)."""
+        n = C.c_int64()
+        self._check(self.lib.wva_grid_update(self.ctx, C.byref(n)), "wva_grid_update")
+        return n.value
+
+    def grid_fetch(self, full: bool = True):
+        """The resident grid: frontier [S, A] and, with full (the grid was run with full outputs), ok / ttft / itl / rho /
+        tput [S, A, R], as analyze_grid returns them."""
+        S, A = self.hi - self.lo, self.A
+        R = self._grid_R
+        n = S * A * R
+        out = {"frontier": np.zeros(max(S * A, 1), dtype=np.int32)}
+        if full:
+            out["ok"] = np.zeros(max(n, 1), dtype=np.uint8)
+            for k in ("ttft", "itl", "rho", "tput"):
+                out[k] = np.zeros(max(n, 1), dtype=np.float32)
+        p = lambda k: out[k].ctypes.data if k in out else None
+        self._check(self.lib.wva_grid_fetch(self.ctx, p("ok"), p("ttft"), p("itl"), p("rho"), p("tput"), p("frontier")),
+                    "wva_grid_fetch")
+        for k in list(out):
+            out[k] = out[k][: S * A].reshape(S, A) if k == "frontier" else out[k][:n].reshape(S, A, R)
+        return out
 
     def grid_fetch_frontier(self):
         S = self.hi - self.lo

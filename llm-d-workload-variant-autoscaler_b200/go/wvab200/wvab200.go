@@ -103,6 +103,17 @@ func (x *Ctx) Recalculate() (resized, revalued int64, err error) {
 	return int64(r), int64(v), err
 }
 
+// GridUpdate brings the replica grid resident from the last wva_grid_run up to date with the UpdateServers calls since
+// then, re-evaluating only the servers whose load changed, with the grid of a full wva_grid_run (INTEGRATION.md §3,
+// per-cycle use).  It returns how many servers of this context's block were re-evaluated.
+func (x *Ctx) GridUpdate() (regridded int64, err error) {
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	var n C.int64_t
+	err = x.err(C.wva_grid_update(x.c, &n), "wva_grid_update")
+	return int64(n), err
+}
+
 // index maps built from SORTED names: ascending index is then a valid Go map order and the
 // name-based tie-breaks of the reference become index comparisons.
 type index struct {
