@@ -35,34 +35,31 @@
 using namespace wva;
 
 // ------------------------------------------------------------------ small helpers
-struct DevBuf {  // growable device allocation
+// growable allocation that its owner frees by being deleted (with the owner's device current): device memory (DevBuf)
+// or pinned host staging (PinBuf)
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct Buf {
   void* p = nullptr;
   size_t cap = 0;
+  Buf() = default;
+  Buf(Buf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  ~Buf() { if (p) Free(p); }
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
+    if (p) Free(p);
     p = nullptr; cap = 0;
     size_t want = n + n / 8 + 256;
-    cudaError_t e = cudaMalloc(&p, want);
+    cudaError_t e = Alloc(&p, want);
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
-struct PinBuf {  // growable pinned host staging
-  void* p = nullptr;
-  size_t cap = 0;
-  cudaError_t reserve(size_t n) {
-    if (n <= cap) return cudaSuccess;
-    if (p) cudaFreeHost(p);
-    p = nullptr; cap = 0;
-    size_t want = n + n / 8 + 256;
-    cudaError_t e = cudaMallocHost(&p, want);
-    if (e == cudaSuccess) cap = want;
-    return e;
-  }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-};
+inline cudaError_t dev_alloc(void** p, size_t n) { return cudaMalloc(p, n); }
+inline cudaError_t pin_alloc(void** p, size_t n) { return cudaMallocHost(p, n); }
+using DevBuf = Buf<dev_alloc, cudaFree>;
+using PinBuf = Buf<pin_alloc, cudaFreeHost>;
 
 // ------------------------------------------------------------------ column lists
 // Every struct-of-arrays of the C-ABI is declared once, in the order its arena is laid out: X(field, count, flags).  The
@@ -70,7 +67,8 @@ struct PinBuf {  // growable pinned host staging
 // them: each_<list>(n, f, s...) calls f(count, flags, s.field...) for every column.  Element sizes come from the fields.
 // Counts are written over the extents `n`; over the entities BEFORE a block (servers before a rank's block, models /
 // variants / replicas before a group member's block) a column's count is its offset to that block.
-struct Ext { size_t A = 0, T = 0, M = 0, S = 0, V = 0, P = 0, R = 0; };   // P: pairs or replicas, R: grid levels
+struct Ext { size_t A = 0, T = 0, M = 0, S = 0, V = 0, P = 0, R = 0, N = 0; };   // P: pairs or replicas, R: grid levels,
+                                                                                // N: capacity-store slots
 enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL too
        COL_DETAIL = 2,    // V1 saturation analysis field: written only by a detail run
        COL_CYCLE = 4 };   // server column wva_update_servers replaces in place (ServerLoadSpec and CurrentAlloc)
@@ -120,6 +118,38 @@ enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL t
 // the replica grid's optional outputs (wva_grid_run with full != 0)
 #define GRID_COLS(X)                                                                                                   \
   X(ok, n.P * n.R, 0) X(ttft, n.P * n.R, 0) X(itl, n.P * n.R, 0) X(rho, n.P * n.R, 0) X(tput, n.P * n.R, 0)
+// The ingest arenas (wva_ingest_create / wva_ingest_v2_create), over S pod slots and N store slots: the caller's host
+// image and the device image of each arena share the offsets.  The decision-mode lists follow the plain ones in the
+// same arenas.
+#define INGEST_COLS(X) X(kv, n.S, 0) X(queue, n.S, 0) X(has, n.S, 0) SAT_IN_SHARED_COLS(X)
+#define INGEST_RES_COLS(X)                                                                                             \
+  X(partials, 8, 0) X(var_target, n.V, 0) X(var_replica_count, n.V, 0) X(var_non_saturated, n.V, 0)                  \
+  X(var_avg_spare_kv, n.V, 0) X(var_avg_spare_queue, n.V, 0) X(mod_flags, n.M, 0) X(mod_total_replicas, n.M, 0)
+#define INGEST_DEC_COLS(X)                                                                                             \
+  X(var_accelerator_type, n.V, 0) X(var_gpus_per_replica, n.V, 0) X(mod_scale_to_zero_enabled, n.M, 0)                \
+  X(mod_request_count, n.M, 0) X(mod_request_error, n.M, 0) X(type_limit, n.T + 1, 0) X(enable_limiter, 1, 0)
+#define INGEST_DEC_RES_COLS(X)                                                                                         \
+  X(has_decision, n.V, 0) X(original_target, n.V, 0) X(target, n.V, 0) X(gpus_allocated, n.V, 0)                     \
+  X(was_limited, n.V, 0) X(action, n.V, 0) X(mod_enforcer_applied, n.M, 0)
+#define INGEST_V2_COLS(X)                                                                                              \
+  X(kv, n.S, 0) X(queue, n.S, 0) X(num_gpu_blocks, n.S, 0) X(block_size, n.S, 0) X(avg_output_tokens, n.S, 0)         \
+  X(avg_input_tokens, n.S, 0) X(prefix_hit_rate, n.S, 0) X(has, n.S, 0) X(var_cost, n.V, 0) X(var_current, n.V, 0)    \
+  X(var_pending, n.V, 0) X(var_name_rank, n.V, 0) X(cfg_kv_threshold, n.M, 0) X(cfg_queue_threshold, n.M, 0)          \
+  X(cfg_scale_up_threshold, n.M, 0) X(cfg_scale_down_boundary, n.M, 0) X(mod_scale_to_zero_enabled, n.M, 0)           \
+  X(mod_request_count, n.M, 0) X(mod_request_error, n.M, 0) X(slot_max_batched_tokens, n.N, 0)                        \
+  X(slot_max_num_seqs, n.N, 0)
+// the analyze launch's results (the replica columns hold every slot, with room to spare)
+#define INGEST_V2_ANALYZE_COLS(X)                                                                                      \
+  X(variant_replica_off, n.V + 2, 0) X(rep_pod, n.S + 4, 0) X(rep_total_kv_tokens, n.S + 2, 0)                        \
+  X(slot_last_rep, n.N, 0) X(slot_effective, n.N, 0) X(var_no_data, n.V, 0) X(mod_has_request, n.M, 0)               \
+  X(mod_avg_input_tokens, n.M, 0) X(mod_avg_output_tokens, n.M, 0)
+// the decide launch's results: its own, then the analyzer's outputs (SatV2Out's fields)
+#define INGEST_V2_DECIDE_COLS(X)                                                                                       \
+  X(var_optimizer_target, n.V, 0) X(var_target, n.V, 0) X(var_action, n.V, 0) X(mod_enforced, n.M, 0)
+#define INGEST_V2_DECIDE_SAT_COLS(X)                                                                                   \
+  X(var_ready, n.V, 0) X(var_per_replica_capacity, n.V, 0) X(var_total_capacity, n.V, 0) X(var_total_demand, n.V, 0)  \
+  X(var_utilization, n.V, 0) X(mod_total_supply, n.M, 0) X(mod_total_demand, n.M, 0) X(mod_utilization, n.M, 0)       \
+  X(mod_required_capacity, n.M, 0) X(mod_spare_capacity, n.M, 0)
 
 #define COL_VISIT_(field, count, flags) f((size_t)(count), flags, s.field...);
 #define COL_VISITOR_(name, LIST) \
@@ -133,6 +163,14 @@ COL_VISITOR_(each_sat_out, SAT_OUT_COLS)
 COL_VISITOR_(each_v2_in, V2_IN_COLS)
 COL_VISITOR_(each_v2_out, V2_OUT_COLS)
 COL_VISITOR_(each_grid, GRID_COLS)
+COL_VISITOR_(each_ingest, INGEST_COLS)
+COL_VISITOR_(each_ingest_res, INGEST_RES_COLS)
+COL_VISITOR_(each_ingest_dec, INGEST_DEC_COLS)
+COL_VISITOR_(each_ingest_dec_res, INGEST_DEC_RES_COLS)
+COL_VISITOR_(each_ingest_v2, INGEST_V2_COLS)
+COL_VISITOR_(each_ingest_v2_analyze, INGEST_V2_ANALYZE_COLS)
+COL_VISITOR_(each_ingest_v2_decide, INGEST_V2_DECIDE_COLS)
+COL_VISITOR_(each_ingest_v2_decide_sat, INGEST_V2_DECIDE_SAT_COLS)
 #undef COL_VISITOR_
 #undef COL_VISIT_
 
@@ -207,6 +245,30 @@ template <class F, class Lay> static cudaError_t lay_out(DevBuf& buf, F& f, Lay&
   return e;
 }
 
+// Lays out an arena that has a page-locked host image and a device image at the same offsets: f(count, flags, host
+// field, device field) binds both to the column.  The two fields may differ in type, not in element size.
+struct Twin : Layout {
+  char* host = nullptr;
+  template <class T, class U> void operator()(size_t n, int, T*& h, U*& d) {
+    static_assert(sizeof(T) == sizeof(U), "one element size in both images");
+    const size_t o = take(n * sizeof(T));
+    if (base) { h = (T*)(host + o); d = (U*)(base + o); }
+  }
+};
+// lay_out for a Twin: the host image (zeroed) and the device image reserved, then every column bound.  Returns the
+// arena's bytes (0 if a reservation fails: `e` says why).
+template <class Lay> static size_t lay_out(PinBuf& hbuf, DevBuf& dbuf, Lay&& lay, cudaError_t& e) {
+  Twin f;
+  lay(f);
+  const size_t bytes = f.off + 256;
+  if ((e = hbuf.reserve(bytes)) != cudaSuccess || (e = dbuf.reserve(bytes)) != cudaSuccess) return 0;
+  memset(hbuf.p, 0, bytes);
+  f = Twin{};
+  f.base = (char*)dbuf.p; f.host = (char*)hbuf.p;
+  lay(f);
+  return bytes;
+}
+
 struct GridState {   // results of the last wva_grid_run, resident in HBM
   int R = 0;
   bool full = false, ran = false;
@@ -260,7 +322,6 @@ struct wva_ctx {
   SizerCounters* d_ctr = nullptr;   // in scratch
   // generic io arenas for saturation / limiter / grid / mm1k
   DevBuf io_in, io_out;
-  PinBuf io_stage_in, io_stage_out;
   GridState grid;
   SatState sat;
   // multi-GPU (comm.inl): one NCCL communicator, contiguous block of servers per rank
@@ -347,11 +408,7 @@ int32_t wva_destroy(wva_ctx* ctx) {
   if (!ctx) return WVA_ERR_ARG;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  ctx->sys_arena.release(); ctx->cand_arena.release(); ctx->sol_arena.release(); ctx->scratch.release();
-  ctx->marks.release(); ctx->grid_marks.release(); ctx->cycle_in.release(); ctx->recalc_ws.release(); ctx->gather_ws.release();
-  ctx->gtab.release(); ctx->pool_ws.release(); ctx->greedy_ws.release(); ctx->split_ws.release(); ctx->order_ws.release(); ctx->grid.buf.release(); ctx->grid.defer.release(); ctx->sat.in.release(); ctx->sat.out.release(); ctx->sat.desc.release(); ctx->io_in.release(); ctx->io_out.release();
-  ctx->stage_in.release(); ctx->stage_out.release(); ctx->io_stage_in.release(); ctx->io_stage_out.release();
-  comm_release(ctx); ctx->comm_ws.release();
+  comm_release(ctx);
   for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
@@ -452,12 +509,9 @@ static cudaError_t launch_sizer(wva_ctx* ctx, const SysView& sys_v, const CandVi
     SplitWs sw = {nullptr, nullptr, nullptr};
     const bool split = ctx->lane_sizer_mode == 4 || ctx->lane_sizer_mode == 5;
     if (split) {
-      size_t need = (size_t)n_pairs * 20 + 256;
-      e = ctx->split_ws.reserve(need);
+      Layout L;
+      e = lay_out(ctx->split_ws, L, [&](Layout& f) { f(2 * n_pairs, 0, sw.res); f(2 * n_pairs, 0, sw.solves); f(n_pairs, 0, sw.cnt); });
       if (e != cudaSuccess) return e;
-      sw.res = (float*)ctx->split_ws.p;
-      sw.solves = (int*)((char*)ctx->split_ws.p + (size_t)n_pairs * 8);
-      sw.cnt = (int*)((char*)ctx->split_ws.p + (size_t)n_pairs * 16);
       e = cudaMemsetAsync(sw.cnt, 0, (size_t)n_pairs * 4, ctx->stream);
       if (e != cudaSuccess) return e;
     }
@@ -475,14 +529,13 @@ static cudaError_t launch_sizer(wva_ctx* ctx, const SysView& sys_v, const CandVi
       size_t tmp = 0;
       cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr,
                                                 (unsigned*)nullptr, (int)n_items, 0, 32, ctx->stream);
-      const size_t arr = ((size_t)n_items * 4 + 255) & ~(size_t)255;
-      e = ctx->order_ws.reserve(4 * arr + tmp + 256);
+      unsigned *k_in = nullptr, *k_out = nullptr, *v_in = nullptr, *v_out = nullptr;
+      unsigned char* d_tmp = nullptr;
+      Layout L;
+      e = lay_out(ctx->order_ws, L, [&](Layout& f) {
+        f(n_items, 0, k_in); f(n_items, 0, k_out); f(n_items, 0, v_in); f(n_items, 0, v_out); f(tmp, 0, d_tmp);
+      });
       if (e != cudaSuccess) return e;
-      unsigned* k_in = (unsigned*)ctx->order_ws.p;
-      unsigned* k_out = (unsigned*)((char*)ctx->order_ws.p + arr);
-      unsigned* v_in = (unsigned*)((char*)ctx->order_ws.p + 2 * arr);
-      unsigned* v_out = (unsigned*)((char*)ctx->order_ws.p + 3 * arr);
-      void* d_tmp = (char*)ctx->order_ws.p + 4 * arr;
       const unsigned pb = (unsigned)((n_items + 127) / 128);
       if (split) sizer_probe_kernel<true><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
       else sizer_probe_kernel<false><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
@@ -554,11 +607,9 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
   const unsigned long long n_pairs = (unsigned long long)sys_v.n_servers * ctx->A;
   // scratch: counters + nmax reduction + overflow list.  The split sizer modes process a pair as TWO items and each may
   // append the pair (both chains of an alpha-dominated pair overflow at lambda_max): 2 entries per pair.
-  size_t need = 256 + 256 + (size_t)n_pairs * 8 + 1024;
-  CK(ctx->scratch.reserve(need));
-  ctx->d_ctr = (SizerCounters*)ctx->scratch.p;
-  int* d_nmax = (int*)((char*)ctx->scratch.p + 256);
-  int* d_ovf = (int*)((char*)ctx->scratch.p + 512);
+  int *d_nmax = nullptr, *d_ovf = nullptr;
+  Layout L;
+  CK(lay_out(ctx->scratch, L, [&](Layout& f) { f(1, 0, ctx->d_ctr); f(1, 0, d_nmax); f(2 * n_pairs + 256, 0, d_ovf); }));
   CK(cudaMemsetAsync(ctx->scratch.p, 0, 512, ctx->stream));
   CK(cudaEventRecord(ctx->ev[2], ctx->stream));
   if (n_pairs > 0) {
@@ -792,13 +843,12 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
     size_t tmp = 0;
     CK(cub::DevicePartition::If(nullptr, tmp, servers, (int*)nullptr, (int*)nullptr, clean, (int*)nullptr, n,
                                 MarkedResize{marks}, MarkedRevalueOnly{marks}, ctx->stream));
-    const size_t list = ((size_t)n * 4 + 255) & ~(size_t)255;
-    CK(ctx->recalc_ws.reserve(2 * list + 256 + tmp));
-    resize = (int*)ctx->recalc_ws.p;
-    revalue = (int*)((char*)ctx->recalc_ws.p + list);
-    int* d_cnt = (int*)((char*)ctx->recalc_ws.p + 2 * list);
-    CK(cub::DevicePartition::If((char*)ctx->recalc_ws.p + 2 * list + 256, tmp, servers, resize, revalue, clean, d_cnt, n,
-                                MarkedResize{marks}, MarkedRevalueOnly{marks}, ctx->stream));
+    int* d_cnt = nullptr;
+    unsigned char* d_tmp = nullptr;
+    Layout L;
+    CK(lay_out(ctx->recalc_ws, L, [&](Layout& f) { f(n, 0, resize); f(n, 0, revalue); f(2, 0, d_cnt); f(tmp, 0, d_tmp); }));
+    CK(cub::DevicePartition::If(d_tmp, tmp, servers, resize, revalue, clean, d_cnt, n, MarkedResize{marks},
+                                MarkedRevalueOnly{marks}, ctx->stream));
     ctx->launches++;
     CK(cudaMemsetAsync(ctx->marks.p, 0, ctx->S, ctx->stream));
     CK(cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
@@ -876,17 +926,20 @@ static int32_t solve_view(wva_ctx* ctx, const SysView& sv, const CandView& cv, c
   // AllocateByType
   int nparts = (S + 255) / 256;
   if (nparts < 1) nparts = 1;
-  size_t need = (size_t)nparts * (T > 0 ? T : 1) * 16 + 512;
+  const size_t n_part = (size_t)nparts * (T > 0 ? T : 1);
   // reuse scratch beyond its first 1024 bytes (counters)
-  CK(ctx->scratch.reserve(1024 + need));
-  long long* pc = (long long*)((char*)ctx->scratch.p + 1024);
-  double* pd = (double*)((char*)ctx->scratch.p + 1024 + (size_t)nparts * (T > 0 ? T : 1) * 8);
+  unsigned char* counters = nullptr;
+  long long* pc = nullptr;
+  double* pd = nullptr;
+  Layout L;
+  CK(lay_out(ctx->scratch, L, [&](Layout& f) { f(1024, 0, counters); f(n_part, 0, pc); f(n_part, 0, pd); }));
   if (T > 0) {
     if (S > 0) {
       by_type_partial_kernel<<<nparts, 256, 0, ctx->stream>>>(sv, ov, pc, pd);
       ctx->launches++;
     } else {
-      CK(cudaMemsetAsync(pc, 0, need - 512, ctx->stream));
+      CK(cudaMemsetAsync(pc, 0, n_part * 8, ctx->stream));
+      CK(cudaMemsetAsync(pd, 0, n_part * 8, ctx->stream));
     }
     by_type_final_kernel<<<T, 256, 0, ctx->stream>>>(T, S > 0 ? nparts : 0, pc, pd, ctx->d_type_count, ctx->d_type_cost);
     ctx->launches++;
