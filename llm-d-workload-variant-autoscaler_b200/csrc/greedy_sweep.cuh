@@ -33,6 +33,7 @@ __device__ __forceinline__ unsigned ge_flags(unsigned meta) { return (meta >> 8)
 __device__ __forceinline__ int ge_rank(unsigned meta) { return (int)(meta >> 16); }
 
 constexpr int GSW_BLOCK = 512;            // events per ring slot (8 KB)
+constexpr int GSW_AVAIL = 64;             // capacity types (WVA_MAX_TYPES)
 
 struct GSweepWs {
   // dense, indexed (server, rank): tau components and flags of every potential event
@@ -44,6 +45,15 @@ struct GSweepWs {
   int* stamp;        // [S] clock of the entry's last failure
   int* dyn_pos; int* dyn_stamp;   // [S] scratch of the tie-group procedure
   unsigned long long* blk_min;    // [n_blocks + 1][n_types] smallest unit count among the events of type t at or after the block
+  // the head of the list (gsw_head_kernel): units of type t wanted by the first candidates (rank 0) in a block, then
+  // the exclusive prefix of those sums over the blocks
+  long long* blk_sum;             // [n_blocks + 1][n_types]
+  long long* head_used;           // [n_types] units the committed head takes from each type
+  unsigned* head_alive;           // [(S + 31) / 32] alive bits after the head
+  // [0] first block some type runs out in, [1] first block the sweep's nothing-fits check stops at (both per type, then
+  // min / max over the types), [2] P: first failure, [3] C: end of the head (events [0, C) are committed in parallel)
+  int* head;
+  unsigned long long* head_events;   // first candidates committed (the sweep's n_active at C)
 };
 
 // tau, run class and flags of every (server, rank); after greedy_prepare_kernel
@@ -65,6 +75,11 @@ __global__ void __launch_bounds__(128) gsw_events_kernel(SysView s, GreedyWs w, 
   }
   for (int j = n; j < A; j++) g.valid[p + j] = 0;
   g.stamp[srv] = 0;
+  if ((srv & 31) == 0) g.head_alive[srv >> 5] = ~0u;
+  if (srv == 0) {
+    for (int t = 0; t < s.n_types; t++) g.head_used[t] = 0;
+    g.head[0] = INT_MAX; g.head[1] = 0; g.head[2] = 0; g.head[3] = 0; *g.head_events = 0;
+  }
 }
 
 // one LSD radix pass over the compacted events: which = 0 run class (re-inserted first), 1 tau value, 2 tau delta, 3 priority
@@ -100,7 +115,11 @@ __global__ void __launch_bounds__(256) gsw_gather_kernel(SysView s, GreedyWs w, 
   e.meta = (unsigned)(ty < 0 ? 0xff : ty) | (flags << 8) | ((unsigned)j << 16);
   e.cnt = (long long)w.r_nrep[p] * w.r_upr[p];
   g.ev[i] = e;
-  if (ty >= 0) atomicMin(&g.blk_min[(size_t)(i / GSW_BLOCK) * s.n_types + ty], (unsigned long long)e.cnt);
+  if (ty >= 0) {
+    const size_t r = (size_t)(i / GSW_BLOCK) * s.n_types + ty;
+    atomicMin(&g.blk_min[r], (unsigned long long)e.cnt);
+    if (j == 0) atomicAdd(reinterpret_cast<unsigned long long*>(&g.blk_sum[r]), (unsigned long long)e.cnt);
+  }
 }
 
 // suffix minima over the blocks: one warp per type, 32 blocks per step (warp suffix scan + carry)
@@ -119,6 +138,122 @@ __global__ void __launch_bounds__(32) gsw_sufmin_kernel(GSweepWs g, int n_blocks
     if (b >= 0) g.blk_min[(size_t)b * n_types + t] = v;
     carry = __shfl_sync(0xffffffffu, v, 31);
   }
+}
+
+// The head of the list.  Event (e, j >= 1) can only be alive after (e, j-1) failed, and a failure needs avail[t] < cnt;
+// so up to the first failure P every alive event is an entry's first candidate (rank 0), taken or — no accelerator —
+// dropped, and every other event is dead.  Before P no stamp is drawn (the clock stays 0), no entry is unallocated and
+// no MULTI leader is alive (MULTI marks re-inserted leaders only, rank >= 1), so a priority boundary runs bestEffort on
+// an empty list.  The only state the head passes on is the units it takes from each type: P is the first event of rank 0
+// and type t >= 0 at which the running sum of those units over the list's rank-0 events of type t exceeds the capacity.
+// The sweep's nothing-fits check (per block, against the capacities at the block's first event) can also stop the
+// sweep before P; the head ends at C = min(P, the first block start where that check stops it), the sweep starts at C
+// with the state the sequential sweep had there, and checks the blocks from C's on as it always did.  (Unit counts
+// are >= 0, as the check's unsigned block minima already assume: the running sums only grow.)
+
+// per type, one warp, 32 blocks per step: blk_sum -> exclusive prefix over the blocks; the first block in which the type
+// runs out (head[0], min over the types) and the first block whose nothing-fits check finds no event of the type that
+// fits, assuming nothing failed before it (head[1], max over the types: the check stops where every type is past it;
+// before P both terms only move one way, so "nothing fits at block b" is "b >= every type's block")
+__global__ void __launch_bounds__(32) gsw_prefix_kernel(SysView s, GSweepWs g, int n_blocks) {
+  const unsigned full = 0xffffffffu;
+  const int t = blockIdx.x, lane = threadIdx.x, T = s.n_types;
+  if (t >= T) return;
+  const long long cap = s.type_count[t];
+  long long carry = 0;
+  int out = INT_MAX, stop = n_blocks;
+  for (int b0 = 0; b0 < n_blocks; b0 += 32) {
+    const int b = b0 + lane;
+    const size_t r = (size_t)b * T + t;
+    const long long v = b < n_blocks ? g.blk_sum[r] : 0;
+    long long incl = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const long long u = __shfl_up_sync(full, incl, o);
+      if (lane >= o) incl += u;
+    }
+    incl += carry;
+    bool can = true;
+    if (b < n_blocks) {
+      const long long left = cap - (incl - v);      // the sweep's avail[t] at the block's first event
+      const unsigned long long m = g.blk_min[r];
+      can = m != ~0ull && left >= 0 && (unsigned long long)left >= m;
+      g.blk_sum[r] = incl - v;
+    }
+    const unsigned runs = __ballot_sync(full, b < n_blocks && incl > cap), cant = __ballot_sync(full, !can);
+    if (runs && out == INT_MAX) out = b0 + __ffs(runs) - 1;
+    if (cant && stop == n_blocks) stop = b0 + __ffs(cant) - 1;
+    carry = __shfl_sync(full, incl, 31);
+  }
+  if (lane == 0) {
+    if (out != INT_MAX) atomicMin(&g.head[0], out);
+    atomicMax(&g.head[1], stop);
+  }
+}
+
+// adds the units of the rank-0 events in [i0, end) (one block at most) to used[type], in order, 32 per step; returns
+// the first of them that does not fit (end if all do)
+__device__ __forceinline__ int gsw_head_walk(const SysView& s, const GSweepWs& g, long long* used, int i0, int end) {
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  for (int b0 = i0; b0 < end; b0 += 32) {
+    const int i = b0 + lane;
+    int ty = -1;
+    long long c = 0;
+    if (i < end) {
+      const GEvent e = g.ev[i];
+      if (ge_rank(e.meta) == 0) { ty = ge_type(e.meta); c = e.cnt; }
+    }
+    long long acc = 0;                               // units of this type in the step, up to and including this lane
+    for (int k = 0; k < 32; k++) {
+      const int tk = __shfl_sync(full, ty, k);
+      const long long ck = __shfl_sync(full, c, k);
+      if (k <= lane && tk == ty) acc += ck;
+    }
+    const unsigned fm = __ballot_sync(full, ty >= 0 && used[ty] + acc > s.type_count[ty]);
+    if (fm) return b0 + __ffs(fm) - 1;
+    const unsigned later = __match_any_sync(full, ty) & ~((2u << lane) - 1u);
+    __syncwarp();
+    if (ty >= 0 && !later) used[ty] += acc;
+    __syncwarp();
+  }
+  return end;
+}
+
+// P and C (head[2], head[3]) and the units the head takes from each type
+__global__ void __launch_bounds__(32) gsw_head_kernel(SysView s, GSweepWs g, int n) {
+  __shared__ long long used[GSW_AVAIL];
+  const int lane = threadIdx.x, T = s.n_types;
+  const int fb = g.head[0];
+  int P = n;
+  if (fb != INT_MAX) {
+    for (int t = lane; t < T; t += 32) used[t] = g.blk_sum[(size_t)fb * T + t];
+    __syncwarp();
+    P = gsw_head_walk(s, g, used, fb * GSW_BLOCK, min(n, (fb + 1) * GSW_BLOCK));
+    __syncwarp();
+  }
+  const int C = min(P, min(g.head[1] * GSW_BLOCK, n)), cb = C / GSW_BLOCK;
+  for (int t = lane; t < T; t += 32) used[t] = g.blk_sum[(size_t)cb * T + t];
+  __syncwarp();
+  gsw_head_walk(s, g, used, cb * GSW_BLOCK, C);
+  __syncwarp();
+  for (int t = lane; t < T; t += 32) g.head_used[t] = used[t];
+  if (lane == 0) { g.head[2] = P; g.head[3] = C; }
+}
+
+// the head, in parallel: every rank-0 event before C is taken (type >= 0) or dropped, and its entry leaves the queue
+__global__ void __launch_bounds__(256) gsw_commit_kernel(GreedyWs w, GSweepWs g, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool first = false;
+  if (i < n && i < g.head[3]) {
+    const GEvent e = g.ev[i];
+    if (ge_rank(e.meta) == 0) {
+      first = true;
+      if (ge_type(e.meta) >= 0) { w.kind[e.srv] = 1; w.sel_rank[e.srv] = 0; }   // greedy.go:143-145
+      atomicAnd(&g.head_alive[e.srv >> 5], ~(1u << (e.srv & 31)));
+    }
+  }
+  const int k = __syncthreads_count(first);
+  if (threadIdx.x == 0 && k) atomicAdd(g.head_events, (unsigned long long)k);
 }
 
 // MULTI: the event leads a re-inserted run and its tie group holds another re-inserted leader.  Bounded walks; when a
@@ -165,7 +300,6 @@ constexpr int GSW_ALIVE_WORDS = 36 * 1024; // alive bits for up to 1 179 648 ent
 constexpr int GSW_TIE_CAP = 1024;          // events of a tie group staged in shared memory at a time
 constexpr int GSW_DYN_CAP = 4096;          // alive leaders of a tie group ordered in shared memory (more: global-memory path)
 constexpr int GSW_RUN_SLOTS = 8;           // runs of a tie group in flight (32 events each, in the staging area)
-constexpr int GSW_AVAIL = 64;              // capacity types (WVA_MAX_TYPES)
 constexpr size_t GSW_SMEM = (size_t)GSW_BLOCK * GSW_SLOTS * sizeof(GEvent) + (size_t)GSW_ALIVE_WORDS * 4 + GSW_AVAIL * 8 +
                             (size_t)GSW_TIE_CAP * sizeof(GEvent) + (size_t)GSW_DYN_CAP * 8;
 
@@ -409,10 +543,12 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
   const unsigned lt = (1u << lane) - 1u;
   const int n_ev = *g.n_events;
   const int S = s.n_servers;
-  for (int t = lane; t < GSW_AVAIL; t += 32) avail[t] = t < s.n_types ? s.type_count[t] : 0;   // greedy.go:38-39
-  for (int k = lane; k < (S + 31) / 32; k += 32) alive[k] = 0xffffffffu;
+  // the sweep starts where the head (gsw_commit_kernel) ends, in the state the sequential sweep had there
+  const int head_end = g.head[3];
+  for (int t = lane; t < GSW_AVAIL; t += 32) avail[t] = t < s.n_types ? s.type_count[t] - g.head_used[t] : 0;   // greedy.go:38-39
+  for (int k = lane; k < (S + 31) / 32; k += 32) alive[k] = g.head_alive[k];
   __syncwarp();
-  GSweepState z = {0, 0, 0, 0, 0, 0, 0};
+  GSweepState z = {0, 0, (long long)*g.head_events, 0, 0, 0, 0};
   int group_un0 = 0;
   long long n_batches = 0, n_rounds = 0, n_seq = 0, n_tie = 0, cyc_be = 0, cyc_tie = 0, n_unalloc_be = 0;
   long long n_tie_global = 0, n_restart = 0;   // tie groups ordered in global memory; event streams restarted after a jump
@@ -420,11 +556,14 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
 
   // event stream: blocks of GSW_BLOCK records copied asynchronously into a ring of GSW_SLOTS slots; while block b is
   // read, blocks b+1 .. b+GSW_SLOTS-1 are in flight.  One commit group per block (empty past the end of the list).
-  int origin = 0;               // event index of block 0 of the current stream (changes only after a far tie-group jump)
+  // The stream starts at the block of the head's end, so that the batches from the next block on (and the block checks)
+  // fall where they fell in a sweep from event 0.  A head that ends inside a block stopped at P, after that block's
+  // nothing-fits check had passed at its first event (gsw_head_kernel): the check is not repeated.
+  int origin = head_end - head_end % GSW_BLOCK;   // event index of block 0 of the current stream (moves only after a far tie-group jump)
   int issued = 0;               // blocks of the current stream whose copies have been issued
   int cur_block = -1;
-  int pos = 0;
-  int checked_blk = -1;
+  int pos = head_end;
+  int checked_blk = head_end % GSW_BLOCK ? head_end / GSW_BLOCK : -1;
   bool nothing_fits = false;
   int pf_blk = -1;
   unsigned long long pf0 = ~0ull, pf1 = ~0ull;
@@ -686,7 +825,7 @@ __global__ void __launch_bounds__(32, 1) gsw_sweep_kernel(SysView s, GreedyWs w,
     g_best_effort(s, w, avail, w.unalloc + group_un0, z.n_un - group_un0, policy, be_stage);
     cyc_be += GSW_CLK() - c0; n_unalloc_be += z.n_un - group_un0;
   }
-  if (lane == 0) { w.stats[8] = cyc_be; w.stats[9] = cyc_tie; w.stats[10] = GSW_CLK() - cyc0; w.stats[11] = n_unalloc_be; w.stats[12] = z.d_fb; w.stats[13] = z.d_nact; w.stats[14] = z.d_maxact; w.stats[15] = z.d_fbev; w.stats[16] = cyc_chk; w.stats[17] = cyc_ring; w.stats[18] = cyc_dead; w.stats[19] = cyc_fast; w.stats[20] = cyc_slow; w.stats[21] = n_survivors; w.stats[22] = n_tie_global; w.stats[23] = n_skip128; w.stats[24] = n_restart; }
+  if (lane == 0) { w.stats[8] = cyc_be; w.stats[9] = cyc_tie; w.stats[10] = GSW_CLK() - cyc0; w.stats[11] = n_unalloc_be; w.stats[12] = z.d_fb; w.stats[13] = z.d_nact; w.stats[14] = z.d_maxact; w.stats[15] = z.d_fbev; w.stats[16] = cyc_chk; w.stats[17] = cyc_ring; w.stats[18] = cyc_dead; w.stats[19] = cyc_fast; w.stats[20] = cyc_slow; w.stats[21] = n_survivors; w.stats[22] = n_tie_global; w.stats[23] = n_skip128; w.stats[24] = n_restart; w.stats[25] = g.head[2]; w.stats[26] = (long long)*g.head_events; w.stats[27] = head_end; }
   if (lane == 0) { w.stats[0] = 0; w.stats[1] = z.n_active; w.stats[2] = n_batches; w.stats[3] = n_rounds; w.stats[4] = n_seq; w.stats[5] = n_tie; w.stats[6] = pos; w.stats[7] = n_ev; }
 }
 
@@ -707,7 +846,9 @@ static inline int32_t run_solve_greedy_sweep(const SysView& s, const CandView& c
                e_ka = etake(P * 4), e_kb = etake(P * 4), e_ne = etake(64), e_ev = etake(P * sizeof(GEvent) + 64), e_st = etake(S * 4),
                e_dp = etake(S * 4), e_ds = etake(S * 4);
   const size_t n_blocks_max = P / GSW_BLOCK + 2;
-  const size_t e_bm = etake(n_blocks_max * (size_t)(s.n_types > 0 ? s.n_types : 1) * 8);
+  const size_t row_bytes = (size_t)(s.n_types > 0 ? s.n_types : 1) * 8;
+  const size_t e_bm = etake(n_blocks_max * row_bytes), e_bs = etake(n_blocks_max * row_bytes), e_hu = etake(GSW_AVAIL * 8),
+               e_ha = etake((S + 31) / 32 * 4), e_hd = etake(4 * 4), e_he = etake(8);
   GreedyWs w;
   size_t tmp = 0;
   void* d_tmp = nullptr;
@@ -721,7 +862,8 @@ static inline int32_t run_solve_greedy_sweep(const SysView& s, const CandView& c
   g.idxA = (unsigned*)(ex + e_ia); g.idxB = (unsigned*)(ex + e_ib); g.keyA = (unsigned*)(ex + e_ka); g.keyB = (unsigned*)(ex + e_kb);
   g.n_events = (int*)(ex + e_ne); g.ev = (GEvent*)(ex + e_ev); g.stamp = (int*)(ex + e_st); g.dyn_pos = (int*)(ex + e_dp);
   g.dyn_stamp = (int*)(ex + e_ds);
-  g.blk_min = (unsigned long long*)(ex + e_bm);
+  g.blk_min = (unsigned long long*)(ex + e_bm); g.blk_sum = (long long*)(ex + e_bs); g.head_used = (long long*)(ex + e_hu);
+  g.head_alive = (unsigned*)(ex + e_ha); g.head = (int*)(ex + e_hd); g.head_events = (unsigned long long*)(ex + e_he);
   if (cudaFuncSetAttribute(gsw_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GSW_SMEM) != cudaSuccess) return WVA_ERR_CUDA;
   const unsigned sb = (unsigned)((S + 127) / 128);
   if (cudaMemsetAsync(w.min_upr, 0x7f, 64 * 8, stream) != cudaSuccess) return WVA_ERR_CUDA;
@@ -746,23 +888,33 @@ static inline int32_t run_solve_greedy_sweep(const SysView& s, const CandView& c
       *launches += 2;
     }
     const int n_blocks = n / GSW_BLOCK + 1;
-    if (cudaMemsetAsync(g.blk_min, 0xff, (size_t)n_blocks * (size_t)(s.n_types > 0 ? s.n_types : 1) * 8, stream) != cudaSuccess) return WVA_ERR_CUDA;
+    if (cudaMemsetAsync(g.blk_min, 0xff, (size_t)n_blocks * row_bytes, stream) != cudaSuccess ||
+        cudaMemsetAsync(g.blk_sum, 0, (size_t)n_blocks * row_bytes, stream) != cudaSuccess) return WVA_ERR_CUDA;
     gsw_gather_kernel<<<cb, 256, 0, stream>>>(s, w, g, cur, n);
     gsw_multi_kernel<<<cb, 256, 0, stream>>>(g, n);
-    if (s.n_types > 0) gsw_sufmin_kernel<<<s.n_types, 32, 0, stream>>>(g, n_blocks, s.n_types);
-    *launches += 3;
+    *launches += 2;
+    if (s.n_types > 0) {
+      gsw_sufmin_kernel<<<s.n_types, 32, 0, stream>>>(g, n_blocks, s.n_types);
+      gsw_prefix_kernel<<<s.n_types, 32, 0, stream>>>(s, g, n_blocks);
+      *launches += 2;
+    }
+    // the head: up to the first failure (or the first block the nothing-fits check stops at), committed in parallel
+    gsw_head_kernel<<<1, 32, 0, stream>>>(s, g, n);
+    gsw_commit_kernel<<<cb, 256, 0, stream>>>(w, g, n);
+    *launches += 2;
   }
   gsw_sweep_kernel<<<1, 32, GSW_SMEM, stream>>>(s, w, g, delayed, policy);
   greedy_finalize_kernel<<<(unsigned)((S + 255) / 256), 256, 0, stream>>>(s, c, o, w);
   *launches += 2;
   if (stats_out) {
-    long long h[25];
-    if (cudaMemcpyAsync(h, w.stats, 200, cudaMemcpyDeviceToHost, stream) != cudaSuccess) return WVA_ERR_CUDA;
+    long long h[28];
+    if (cudaMemcpyAsync(h, w.stats, sizeof(h), cudaMemcpyDeviceToHost, stream) != cudaSuccess) return WVA_ERR_CUDA;
     if (cudaStreamSynchronize(stream) != cudaSuccess) return WVA_ERR_CUDA;
     stats_out[0] = h[0]; stats_out[1] = h[1];
     if (getenv("WVA_SIZER_DEBUG"))
-      fprintf(stderr, "greedy sweep: alive events %lld, batches %lld, rounds %lld, sequential events %lld, tie-group calls %lld, stopped at %lld of %lld; cycles: best effort %lld (%lld entries), tie groups %lld, kernel %lld; tie groups: %lld over the staging size (%lld events), %lld in global memory, alive leaders %lld (max %lld); loop cycles: early-exit check %lld, ring %lld, dead batches %lld, fast path %lld, slow path %lld; entries swept on after nothing fits: %lld; 128-event skips %lld; stream restarts %lld\n",
-              h[1], h[2], h[3], h[4], h[5], h[6], h[7], h[8], h[11], h[9], h[10], h[12], h[15], h[22], h[13], h[14], h[16], h[17], h[18], h[19], h[20], h[21], h[23], h[24]);
+      fprintf(stderr, "greedy sweep: alive events %lld, batches %lld, rounds %lld, sequential events %lld, tie-group calls %lld, stopped at %lld of %lld; cycles: best effort %lld (%lld entries), tie groups %lld, kernel %lld; tie groups: %lld over the staging size (%lld events), %lld in global memory, alive leaders %lld (max %lld); loop cycles: early-exit check %lld, ring %lld, dead batches %lld, fast path %lld, slow path %lld; entries swept on after nothing fits: %lld; 128-event skips %lld; stream restarts %lld; head: first failure at %lld, %lld first candidates committed in parallel, swept from %lld to %lld\n",
+              h[1], h[2], h[3], h[4], h[5], h[6], h[7], h[8], h[11], h[9], h[10], h[12], h[15], h[22], h[13], h[14], h[16], h[17], h[18], h[19], h[20], h[21], h[23], h[24],
+              h[25], h[26], h[27], h[6]);
   }
   return cudaGetLastError() == cudaSuccess ? WVA_OK : WVA_ERR_CUDA;
 }
