@@ -279,6 +279,30 @@ int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t
  * after wva_load_system until the next wva_calculate, after wva_set_candidates, and after a failed sizing.  Timing as
  * for wva_calculate, with calculate_ms over the whole call; with nothing to re-size sizer_kernel and the counts are 0. */
 int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued);
+/* Replace the server set of the loaded system in place: System.AddServerFromSpec / RemoveServer (pkg/core/system.go)
+ * for a whole cycle's servers at once, with every server column re-specified.  `servers` carries the n_servers (S') new
+ * servers' 15 srv_* columns, in ascending-name order (INTEGRATION.md §3); its accelerator, model, perf, type and
+ * optimizer fields are ignored, the loaded system's tables stay.  prev[i] (may be NULL when S' = 0) is the index of new
+ * server i in the loaded system, or -1 for a new server; old indices that appear nowhere are the removed servers.
+ * WVA_ERR_ARG, with nothing changed, unless every prev entry is in [-1, S), the non-negative ones are strictly
+ * increasing, and the columns pass wva_load_system's server checks (non-NULL, srv_model < M, the srv_cur_acc rule).
+ * WVA_ERR_STATE before wva_load_system, and on a ctx with a communicator unless the set is unchanged (S' = S,
+ * prev[i] = i): its rank blocks cannot move.
+ * Every per-server resident array follows the new set: the server columns, the candidate rows, the resident grid (when
+ * it comes from wva_grid_run / wva_grid_update: levels and frontier) and the pending marks of wva_update_servers; the
+ * solution is void (wva_get_solution is WVA_ERR_STATE until wva_solve).  A new server's candidates are nil
+ * (WVA_ALLOC_NONE, every field 0) and its grid rows not ok with frontier 0, until it is sized or re-gridded.  Each kept
+ * server is compared bitwise with its old row and marked as wva_update_servers marks it, widened to every column:
+ * re-size when a column sizer_setup reads changed (the load, srv_model, max batch, target, SLOs, min replicas,
+ * keepAccelerator, or cur_acc on a server whose keepAccelerator is set before or after), re-value when only the current
+ * allocation changed, nothing when only srv_priority changed; a grid mark when a column the grid reads changed (the
+ * load, srv_model, max batch, target, SLOs).  New servers get both marks.  wva_recalculate and wva_grid_update then
+ * consume the marks as they do after wva_update_servers, with the candidates and grid of wva_load_system +
+ * wva_calculate (+ wva_grid_run) on the new system; wva_set_candidates still rules out wva_recalculate.  When the set
+ * changes, the new arenas are reserved before anything moves (WVA_ERR_NOMEM changes nothing) and swapped in after the
+ * move, so the call needs the old and the new arenas at once: about twice the grid's size with full outputs (2 x 14 GB
+ * for 100 000 servers x 32 accelerators at R = 256).  Timing: h2d_ms covers the whole call. */
+int32_t wva_update_server_set(wva_ctx* ctx, int32_t n_servers, const int32_t* prev /* [S'] */, const wva_system* servers);
 /* Manager.Optimize (pkg/manager/manager.go:21-27): Optimizer.Optimize
  * (pkg/solver/optimizer.go:24-36) -> Solver.Solve (solver.go:32-60) — SolveUnlimited
  * (solver.go:63-79) or SolveGreedy (greedy.go:35-105) — then AllocateByType. */

@@ -30,6 +30,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <utility>
 #include <vector>
 
 using namespace wva;
@@ -45,6 +46,7 @@ struct Buf {
   Buf(Buf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
   Buf(const Buf&) = delete;
   Buf& operator=(const Buf&) = delete;
+  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
   ~Buf() { if (p) Free(p); }
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
@@ -71,17 +73,20 @@ struct Ext { size_t A = 0, T = 0, M = 0, S = 0, V = 0, P = 0, R = 0, N = 0; };  
                                                                                 // N: capacity-store slots
 enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL too
        COL_DETAIL = 2,    // V1 saturation analysis field: written only by a detail run
-       COL_CYCLE = 4 };   // server column wva_update_servers replaces in place (ServerLoadSpec and CurrentAlloc)
+       COL_CYCLE = 4,     // server column wva_update_servers replaces in place (ServerLoadSpec and CurrentAlloc)
+       COL_SRV = 8 };     // server column ([S]): wva_update_server_set replaces the set of them
+#define SRV_CYCLE (COL_SRV | COL_CYCLE)
 
+// The model tables come first and the server columns last: a new server set keeps the arena's prefix as it is.
 #define SYS_COLS(X)                                                                                                    \
   X(acc_cost, n.A, 0) X(acc_multiplicity, n.A, 0) X(acc_type, n.A, 0) X(type_count, n.T, 0)                            \
   X(perf_alpha, n.M * n.A, 0) X(perf_beta, n.M * n.A, 0) X(perf_gamma, n.M * n.A, 0) X(perf_max_batch, n.M * n.A, 0)  \
   X(perf_at_tokens, n.M * n.A, 0) X(perf_acc_count, n.M * n.A, 0) X(perf_present, n.M * n.A, 0)                        \
-  X(srv_model, n.S, 0) X(srv_priority, n.S, 0) X(srv_min_replicas, n.S, 0) X(srv_max_batch, n.S, 0)                    \
-  X(srv_keep_acc, n.S, 0) X(srv_target_present, n.S, 0) X(srv_slo_ttft, n.S, 0) X(srv_slo_itl, n.S, 0)                \
-  X(srv_slo_tps, n.S, 0) X(srv_arrival, n.S, COL_CYCLE) X(srv_in_tokens, n.S, COL_CYCLE)                              \
-  X(srv_out_tokens, n.S, COL_CYCLE) X(srv_cur_acc, n.S, COL_CYCLE) X(srv_cur_replicas, n.S, COL_CYCLE)                 \
-  X(srv_cur_cost, n.S, COL_CYCLE)
+  X(srv_model, n.S, COL_SRV) X(srv_priority, n.S, COL_SRV) X(srv_min_replicas, n.S, COL_SRV)                           \
+  X(srv_max_batch, n.S, COL_SRV) X(srv_keep_acc, n.S, COL_SRV) X(srv_target_present, n.S, COL_SRV)                     \
+  X(srv_slo_ttft, n.S, COL_SRV) X(srv_slo_itl, n.S, COL_SRV) X(srv_slo_tps, n.S, COL_SRV)                              \
+  X(srv_arrival, n.S, SRV_CYCLE) X(srv_in_tokens, n.S, SRV_CYCLE) X(srv_out_tokens, n.S, SRV_CYCLE)                    \
+  X(srv_cur_acc, n.S, SRV_CYCLE) X(srv_cur_replicas, n.S, SRV_CYCLE) X(srv_cur_cost, n.S, SRV_CYCLE)
 #define CAND_COLS(X)                                                                                                   \
   X(state, n.P, 0) X(num_replicas, n.P, 0) X(batch_size, n.P, 0) X(cost, n.P, 0) X(value, n.P, 0) X(itl, n.P, 0)      \
   X(ttft, n.P, 0) X(rho, n.P, 0) X(max_arrv_rate, n.P, 0) X(n_solves, n.P, COL_OPT)
@@ -216,11 +221,18 @@ struct Missing {
   template <class T, class H> void operator()(size_t n, int flags, T*, H* h) { any |= n && !h && !(flags & COL_OPT); }
 };
 
-// visits the per-cycle server columns (COL_CYCLE) of S servers only
-template <class F, class... Structs> static void each_cycle(size_t S, F&& f, Structs&&... s) {
+// visits the server columns of S servers that carry every bit of `flag` (COL_SRV: all of them; COL_CYCLE: the per-cycle
+// ones) and nothing else
+template <int FLAG, class F, class... Structs> static void each_srv(size_t S, F&& f, Structs&&... s) {
   Ext n;
   n.S = S;
-  each_sys(n, [&](size_t c, int flags, auto&&... col) { if (flags & COL_CYCLE) f(c, flags, col...); }, s...);
+  each_sys(n, [&](size_t c, int flags, auto&&... col) { if ((flags & FLAG) == FLAG) f(c, flags, col...); }, s...);
+}
+template <class F, class... Structs> static void each_cycle(size_t S, F&& f, Structs&&... s) {
+  each_srv<COL_CYCLE>(S, f, s...);
+}
+template <class F, class... Structs> static void each_server(size_t S, F&& f, Structs&&... s) {
+  each_srv<COL_SRV>(S, f, s...);
 }
 
 // The preconditions of the per-cycle columns, shared by wva_load_system and wva_update_servers: every array non-NULL
@@ -233,6 +245,17 @@ static const char* check_cycle_columns(const wva_system& s, size_t S, int A) {
   for (size_t i = 0; i < S; i++)
     if (s.srv_cur_acc[i] >= A || s.srv_cur_acc[i] < WVA_CUR_ACC_UNKNOWN) return "srv_cur_acc out of range";
   return nullptr;
+}
+// The preconditions of all server columns, shared by wva_load_system and wva_update_server_set: the per-cycle ones, and
+// every other server array non-NULL with srv_model below M (-1 = unknown model).  Returns the violated rule, or nullptr.
+static const char* check_server_columns(const wva_system& s, size_t S, int A, int M) {
+  Missing miss;
+  SysView none = {};
+  each_server(S, miss, none, s);
+  if (miss.any) return "a required array is NULL";
+  for (size_t i = 0; i < S; i++)
+    if (s.srv_model[i] >= M) return "srv_model out of range";
+  return check_cycle_columns(s, S, A);
 }
 
 // Sizes an arena with a pass of `lay` over a copy of `f` that has no base, reserves it, then runs `lay` over `f` with the
@@ -279,6 +302,18 @@ struct GridState {   // results of the last wva_grid_run, resident in HBM
   int* nmax = nullptr;         // device word of the max batch pass
   GridOverflowList ovf = {};   // the block's float64-overflow list, also used by wva_grid_update
 };
+// Lays out the grid buffer of P pairs at R levels through `f`: the counters, the max batch word, the frontier, the
+// float64-overflow list (grid_kernel.cuh: GridOverflowList; 16 levels per pair on average, as the deferral list) and,
+// with full outputs, the level arrays last.
+template <class F> static void grid_columns(F& f, size_t P, int R, bool full, GridCounters*& ctr, int*& nmax, GridOut& view,
+                                            GridOverflowList& ovf) {
+  const size_t n = P * (size_t)R;
+  ovf.cap = std::min<unsigned long long>({(unsigned long long)n, (unsigned long long)P * 16 + 1024, 0x7fffffffull});
+  Ext levels;
+  levels.P = P; levels.R = (size_t)R;
+  f(1, 0, ctr); f(1, 0, nmax); f(P, 0, view.frontier); f(ovf.cap, 0, ovf.items);
+  if (full) each_grid(levels, f, view);
+}
 struct SatState {    // resident inputs / outputs of the saturation model
   bool uploaded = false, ran = false;
   long long M = 0, V = 0, P = 0;
@@ -439,9 +474,7 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   // validate indices the kernels dereference (after the NULL checks above)
   for (size_t a = 0; a < A; a++)
     if (s->acc_type[a] < 0 || s->acc_type[a] >= (int)T) { ctx->last_error = "wva_load_system: acc_type out of range"; return WVA_ERR_ARG; }
-  for (size_t i = 0; i < S; i++)
-    if (s->srv_model[i] >= (int)M) { ctx->last_error = "wva_load_system: srv_model out of range"; return WVA_ERR_ARG; }
-  if (const char* bad = check_cycle_columns(*s, S, (int)A)) { ctx->last_error = std::string("wva_load_system: ") + bad; return WVA_ERR_ARG; }
+  if (const char* bad = check_server_columns(*s, S, (int)A, (int)M)) { ctx->last_error = std::string("wva_load_system: ") + bad; return WVA_ERR_ARG; }
   // ServiceParms (pkg/analyzer/queueanalyzer.go:33-38) are measured service-time coefficients: finite and >= 0.  A
   // negative or NaN coefficient makes arrival rates negative (QueueModel.Solve's gate, queuemodel.go:31) or NaN and
   // the sizing meaningless; it is rejected here instead of being carried into the kernels.
@@ -780,9 +813,10 @@ int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t
   CK(cudaMemcpyAsync(ctx->cycle_in.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
   if (!ctx->marked) CK(cudaMemsetAsync(ctx->marks.p, 0, S, ctx->stream));
   if (!ctx->grid_marked) CK(cudaMemsetAsync(ctx->grid_marks.p, 0, S, ctx->stream));
-  classify_servers_kernel<<<(unsigned)((S + 255) / 256), 256, 0, ctx->stream>>>(ctx->sys, nu, ctx->shard_lo, ctx->shard_hi,
-                                                                               (unsigned char*)ctx->marks.p,
-                                                                               (unsigned char*)ctx->grid_marks.p);
+  unsigned char *marks = (unsigned char*)ctx->marks.p, *grid_marks = (unsigned char*)ctx->grid_marks.p;
+  classify_servers_kernel<<<(unsigned)((S + 255) / 256), 256, 0, ctx->stream>>>(ctx->sys, nu, ctx->sys, nullptr, ctx->shard_lo,
+                                                                               ctx->shard_hi, marks, grid_marks, marks,
+                                                                               grid_marks);
   ctx->launches++;
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev[1], ctx->stream));
@@ -865,7 +899,7 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
     CandView gcand = {};
     Layout G;
     CK(lay_out(ctx->gather_ws, G, [&](Layout& f) {
-      each_sys(g, [&](size_t c, int fl, auto*& p) { if (c) f(c, fl, p); }, gsys);   // server columns only
+      each_server(D, f, gsys);
       each_cand(g, f, gcand);
     }));
     RowMoves in;
@@ -895,6 +929,162 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
   ctx->calculated = true; ctx->solved = false;
   ctx->sized = true;
   ctx->shard_status = WVA_OK;
+  return WVA_OK;
+}
+
+}  // extern "C"
+
+// Every column of `m` (per elements per row) laid out for the new set of n_rows rows, from the run list d_runs (its count,
+// then the runs' first rows) of `prev`.
+static int32_t launch_reindex(wva_ctx* ctx, const RowMoves& m, const int* prev, const int* d_runs, int n_rows, int per) {
+  if (m.n == 0 || n_rows == 0) return WVA_OK;
+  unsigned long long most = 0;
+  for (int c = 0; c < m.n; c++) most = std::max(most, (unsigned long long)n_rows * per * m.width[c]);
+  constexpr int CHUNKS = 8;
+  const unsigned long long blocks = std::min<unsigned long long>((most + 16 * 256 * CHUNKS - 1) / (16 * 256 * CHUNKS),
+                                                                 (unsigned long long)ctx->sm_count * 8);
+  reindex_rows_kernel<CHUNKS><<<dim3((unsigned)blocks, (unsigned)m.n), 256, 0, ctx->stream>>>(m, prev, d_runs + 1, d_runs,
+                                                                                            n_rows, per);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return WVA_OK;
+}
+
+extern "C" {
+
+int32_t wva_update_server_set(wva_ctx* ctx, int32_t n_servers, const int32_t* prev, const wva_system* servers) {
+  if (!ctx) return WVA_ERR_ARG;
+  if (!ctx->loaded) { ctx->last_error = "wva_update_server_set before wva_load_system"; return WVA_ERR_STATE; }
+  const size_t S = (size_t)ctx->S, A = (size_t)ctx->A;
+  auto bad_arg = [&](const char* why) { ctx->last_error = std::string("wva_update_server_set: ") + why; return WVA_ERR_ARG; };
+  if (n_servers < 0 || !servers) return bad_arg("n_servers < 0 or servers NULL");
+  const size_t S2 = (size_t)n_servers;
+  if (S2 > 0 && !prev) return bad_arg("prev is NULL");
+  bool same = S2 == S;
+  for (size_t i = 0, next = 0; i < S2; i++) {   // next: the least old index the next kept server may have
+    const int p = prev[i];
+    if (p < -1 || p >= (int)S) return bad_arg("prev out of range");
+    if (p >= 0 && (size_t)p < next) return bad_arg("the kept servers' prev entries are not strictly increasing");
+    if (p >= 0) next = (size_t)p + 1;
+    same &= p == (int)i;
+  }
+  if (const char* bad = check_server_columns(*servers, S2, ctx->A, ctx->M)) return bad_arg(bad);
+  if (ctx->world > 1 && !same) {
+    ctx->last_error = "wva_update_server_set: the server set of a ctx with a communicator cannot change";
+    return WVA_ERR_STATE;
+  }
+  CK(cudaSetDevice(ctx->device));
+  // the server columns and prev staged at their offsets of one pinned buffer, one H2D copy
+  SysView nu = ctx->sys;
+  nu.n_servers = (int)S2;
+  int* d_prev = nullptr;
+  Layout L;
+  each_server(S2, L, nu);
+  L(S2, 0, d_prev);
+  const size_t total = L.off + 256;
+  CK(ctx->stage_in.reserve(total));
+  CK(ctx->cycle_in.reserve(total));
+  char* h = (char*)ctx->stage_in.p;
+  L = Layout{(char*)ctx->cycle_in.p};
+  auto stage = [&](size_t c, int, auto*& d, auto* src) { if (c) memcpy(h + L.off, src, c * sizeof(*d)); L(c, 0, d); };
+  each_server(S2, stage, nu, *servers);
+  stage(S2, 0, d_prev, prev);
+  if (same) {
+    // the same set: one classify-and-write pass in place, as wva_update_servers
+    CK(ctx->marks.reserve(S));
+    CK(ctx->grid_marks.reserve(S));
+    CK(cudaEventRecord(ctx->ev[0], ctx->stream));
+    CK(cudaMemcpyAsync(ctx->cycle_in.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
+    unsigned char *marks = (unsigned char*)ctx->marks.p, *grid_marks = (unsigned char*)ctx->grid_marks.p;
+    if (S > 0) {
+      classify_servers_kernel<<<(unsigned)((S + 255) / 256), 256, 0, ctx->stream>>>(
+          ctx->sys, nu, ctx->sys, nullptr, ctx->shard_lo, ctx->shard_hi, ctx->marked ? marks : nullptr,
+          ctx->grid_marked ? grid_marks : nullptr, marks, grid_marks);
+      ctx->launches++;
+    }
+  } else {
+    // A new set (one rank): every arena reserved before anything moves, so that a failed reservation changes nothing
+    GridState& g = ctx->grid;
+    Ext n;
+    n.A = A; n.T = (size_t)ctx->T; n.M = (size_t)ctx->M; n.S = S2; n.P = S2 * A;
+    DevBuf sys_arena, cand_arena, sol_arena, marks_buf, grid_marks_buf, grid_buf;
+    SysView sys = ctx->sys;
+    sys.n_servers = (int)S2;
+    CandView cand = {};
+    SolView sol = {};
+    long long* type_count = nullptr;
+    double* type_cost = nullptr;
+    Layout SL, CL, OL, GL;
+    size_t prefix = 0;   // the model tables: the arena up to its first server column
+    CK(lay_out(sys_arena, SL, [&](Layout& f) {
+      each_sys(n, [&](size_t c, int flags, auto*& p) { if ((flags & COL_SRV) && !prefix) prefix = f.off; f(c, flags, p); }, sys);
+    }));
+    CK(lay_out(cand_arena, CL, [&](Layout& f) { each_cand(n, f, cand); }));
+    CK(lay_out(sol_arena, OL, [&](Layout& f) { each_sol(n, f, sol); f(n.T, 0, type_count); f(n.T, 0, type_cost); }));
+    CK(marks_buf.reserve(S2));
+    CK(grid_marks_buf.reserve(S2));
+    GridCounters* gctr = nullptr;
+    int* gnmax = nullptr;
+    GridOut gview = {};
+    GridOverflowList govf = {};
+    if (g.current) CK(lay_out(grid_buf, GL, [&](Layout& f) { grid_columns(f, n.P, g.R, g.full, gctr, gnmax, gview, govf); }));
+    size_t tmp = 0;
+    CK(cub::DeviceSelect::If(nullptr, tmp, thrust::counting_iterator<int>(0), (int*)nullptr, (int*)nullptr, (int)S2,
+                             RunHead{d_prev}, ctx->stream));
+    int* d_runs = nullptr;
+    unsigned char* d_tmp = nullptr;
+    Layout W;
+    CK(lay_out(ctx->recalc_ws, W, [&](Layout& f) { f(S2 + 1, 0, d_runs); f(tmp, 0, d_tmp); }));
+    CK(cudaEventRecord(ctx->ev[0], ctx->stream));
+    CK(cudaMemcpyAsync(ctx->cycle_in.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
+    // the model tables as they are; every server column through the classify pass, the marks carried over
+    if (prefix) CK(cudaMemcpyAsync(sys_arena.p, ctx->sys_arena.p, prefix, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (S2 > 0) {
+      classify_servers_kernel<<<(unsigned)((S2 + 255) / 256), 256, 0, ctx->stream>>>(
+          ctx->sys, nu, sys, d_prev, 0, (int)S2, ctx->marked ? (const unsigned char*)ctx->marks.p : nullptr,
+          ctx->grid_marked ? (const unsigned char*)ctx->grid_marks.p : nullptr, (unsigned char*)marks_buf.p,
+          (unsigned char*)grid_marks_buf.p);
+      ctx->launches++;
+    }
+    // the runs of prev (count word, then each run's first new row), then the candidate rows and the frontier (A per
+    // server) and the grid levels (A * R per server) moved run by run
+    if (S2 > 0) {
+      CK(cub::DeviceSelect::If(d_tmp, tmp, thrust::counting_iterator<int>(0), d_runs + 1, d_runs, (int)S2, RunHead{d_prev},
+                               ctx->stream));
+      ctx->launches++;
+    }
+    RowMoves rows, lv;
+    each_cand(n, AddMove{rows}, ctx->cand, cand);
+    if (g.current) AddMove{rows}(n.P, 0, g.view.frontier, gview.frontier);
+    Ext gx;
+    gx.P = n.P; gx.R = (size_t)g.R;
+    if (g.current && g.full) each_grid(gx, AddMove{lv}, g.view, gview);
+    int32_t rc = launch_reindex(ctx, rows, d_prev, d_runs, (int)S2, (int)A);
+    if (rc == WVA_OK) rc = launch_reindex(ctx, lv, d_prev, d_runs, (int)S2, (int)A * g.R);
+    if (rc != WVA_OK) return rc;
+    CK(cudaMemsetAsync(sol_arena.p, 0, sol_arena.cap, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));   // nothing reads the old arenas any more
+    std::swap(ctx->sys_arena, sys_arena);
+    std::swap(ctx->cand_arena, cand_arena);
+    std::swap(ctx->sol_arena, sol_arena);
+    std::swap(ctx->marks, marks_buf);
+    std::swap(ctx->grid_marks, grid_marks_buf);
+    ctx->sys = sys; ctx->cand = cand; ctx->sol = sol;
+    ctx->d_type_count = type_count; ctx->d_type_cost = type_cost;
+    if (g.current) {
+      std::swap(g.buf, grid_buf);
+      g.view = gview; g.ctr = gctr; g.nmax = gnmax; g.ovf = govf;
+    } else {
+      g.ran = false;   // a grid of the old set, not brought along: nothing to fetch
+    }
+    ctx->S = (int)S2;
+    ctx->shard_rows = (int)S2; ctx->shard_lo = 0; ctx->shard_hi = (int)S2;
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->ev[1], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));   // the staging buffer is free for the next call
+  ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
+  ctx->marked = true; ctx->grid_marked = true; ctx->solved = false;
   return WVA_OK;
 }
 

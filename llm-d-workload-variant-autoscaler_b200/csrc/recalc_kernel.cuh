@@ -12,36 +12,62 @@
 namespace wva {
 
 // marks[srv] bits, accumulated from update to update until the next wva_calculate / wva_recalculate
-enum { MARK_RESIZE = 1,     // a sizing input changed: the load, or the current accelerator of a keepAccelerator server
+enum { MARK_RESIZE = 1,     // a sizing input changed (sizer_setup): the load, the model, a target or SLO, max batch,
+                            // min replicas, keepAccelerator, or the current accelerator of a keepAccelerator server
        MARK_REVALUE = 2 };  // the current allocation changed: TransitionPenalty (every candidate's value) changed
 
 __device__ __forceinline__ bool bits_differ(float a, float b) { return __float_as_uint(a) != __float_as_uint(b); }
 
-// One pass over the S servers: the bitwise diff of the six per-cycle columns of `nu` against the resident `res`, the
-// write of `nu` over `res`, and the marks of the servers in [lo, hi) (the rank's block; every rank holds every column).
-// grid_marks[srv] = 1 when the load changed: a server's grid rows read no other per-cycle column (grid_setup), and they
-// accumulate until the next wva_grid_run / wva_grid_update, apart from the sizing marks.
-__global__ void classify_servers_kernel(SysView res, SysView nu, int lo, int hi, unsigned char* marks,
-                                        unsigned char* grid_marks) {
+// One pass over the servers of `nu`, the new values of every server column: new server i was server p = prev[i] of the
+// resident columns `res` (prev NULL: p = i, the same set), or is new (p < 0).  The bitwise diff of each kept server's
+// columns against row p, the write of `nu` into `out` (res itself for the same set), and the marks of the servers in
+// [lo, hi) (the rank's block; every rank holds every column): the marks of row p (old_marks, NULL = none) carried over
+// and this diff's added.  grid_marks[i] = 1 when a column grid_setup reads changed (the load, the model, a target or
+// SLO, max batch); they accumulate until the next wva_grid_run / wva_grid_update, apart from the sizing marks.  A new
+// server gets both.  srv_priority is written and marks nothing: only the allocators read it.
+__global__ void classify_servers_kernel(SysView res, SysView nu, SysView out, const int* prev, int lo, int hi,
+                                        const unsigned char* old_marks, const unsigned char* old_grid_marks,
+                                        unsigned char* marks, unsigned char* grid_marks) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= res.n_servers) return;
+  if (i >= nu.n_servers) return;
+  const int p = prev ? prev[i] : i;
+  const int model = nu.srv_model[i], prio = nu.srv_priority[i], minr = nu.srv_min_replicas[i], mb = nu.srv_max_batch[i];
+  const unsigned char keep = nu.srv_keep_acc[i], tp = nu.srv_target_present[i];
+  const float ttft = nu.srv_slo_ttft[i], itl = nu.srv_slo_itl[i], tps = nu.srv_slo_tps[i];
   const float arr = nu.srv_arrival[i], cost = nu.srv_cur_cost[i];
   const int in_tok = nu.srv_in_tokens[i], out_tok = nu.srv_out_tokens[i];
   const int acc = nu.srv_cur_acc[i], rep = nu.srv_cur_replicas[i];
-  const bool load = bits_differ(arr, res.srv_arrival[i]) || in_tok != res.srv_in_tokens[i] ||
-                    out_tok != res.srv_out_tokens[i];
-  const bool acc_moved = acc != res.srv_cur_acc[i];
-  const bool alloc = acc_moved || rep != res.srv_cur_replicas[i] || bits_differ(cost, res.srv_cur_cost[i]);
-  // the candidate set depends on the current accelerator when keepAccelerator is set (server.go:70-82)
-  const bool resize = load || (acc_moved && res.srv_keep_acc[i]);
-  const_cast<float*>(res.srv_arrival)[i] = arr;
-  const_cast<int*>(res.srv_in_tokens)[i] = in_tok;
-  const_cast<int*>(res.srv_out_tokens)[i] = out_tok;
-  const_cast<int*>(res.srv_cur_acc)[i] = acc;
-  const_cast<int*>(res.srv_cur_replicas)[i] = rep;
-  const_cast<float*>(res.srv_cur_cost)[i] = cost;
-  if (i >= lo && i < hi && (resize || alloc)) marks[i] |= (resize ? MARK_RESIZE : 0) | (alloc ? MARK_REVALUE : 0);
-  if (i >= lo && i < hi && load) grid_marks[i] = 1;
+  unsigned char mark = MARK_RESIZE, grid = 1;
+  if (p >= 0) {
+    const bool load = bits_differ(arr, res.srv_arrival[p]) || in_tok != res.srv_in_tokens[p] ||
+                      out_tok != res.srv_out_tokens[p];
+    const bool gridded = load || model != res.srv_model[p] || mb != res.srv_max_batch[p] ||
+                         tp != res.srv_target_present[p] || bits_differ(ttft, res.srv_slo_ttft[p]) ||
+                         bits_differ(itl, res.srv_slo_itl[p]) || bits_differ(tps, res.srv_slo_tps[p]);
+    const bool acc_moved = acc != res.srv_cur_acc[p];
+    const bool alloc = acc_moved || rep != res.srv_cur_replicas[p] || bits_differ(cost, res.srv_cur_cost[p]);
+    // the candidate set depends on the current accelerator when keepAccelerator is set (server.go:70-82)
+    const bool resize = gridded || minr != res.srv_min_replicas[p] || keep != res.srv_keep_acc[p] ||
+                        (acc_moved && (keep || res.srv_keep_acc[p]));
+    mark = (resize ? MARK_RESIZE : 0) | (alloc ? MARK_REVALUE : 0) | (old_marks ? old_marks[p] : 0);
+    grid = (gridded ? 1 : 0) | (old_grid_marks ? old_grid_marks[p] : 0);
+  }
+  const_cast<int*>(out.srv_model)[i] = model;
+  const_cast<int*>(out.srv_priority)[i] = prio;
+  const_cast<int*>(out.srv_min_replicas)[i] = minr;
+  const_cast<int*>(out.srv_max_batch)[i] = mb;
+  const_cast<unsigned char*>(out.srv_keep_acc)[i] = keep;
+  const_cast<unsigned char*>(out.srv_target_present)[i] = tp;
+  const_cast<float*>(out.srv_slo_ttft)[i] = ttft;
+  const_cast<float*>(out.srv_slo_itl)[i] = itl;
+  const_cast<float*>(out.srv_slo_tps)[i] = tps;
+  const_cast<float*>(out.srv_arrival)[i] = arr;
+  const_cast<int*>(out.srv_in_tokens)[i] = in_tok;
+  const_cast<int*>(out.srv_out_tokens)[i] = out_tok;
+  const_cast<int*>(out.srv_cur_acc)[i] = acc;
+  const_cast<int*>(out.srv_cur_replicas)[i] = rep;
+  const_cast<float*>(out.srv_cur_cost)[i] = cost;
+  if (i >= lo && i < hi) { marks[i] = mark; grid_marks[i] = grid; }
 }
 
 // the two lists wva_recalculate compacts from the marks (a re-sized server is re-valued by its sizing already)
@@ -76,6 +102,70 @@ __global__ void move_rows_kernel(RowMoves m, const int* rows, unsigned long long
         case 2: ((short*)m.dst[c])[to] = ((const short*)m.src[c])[from]; break;
         case 4: ((int*)m.dst[c])[to] = ((const int*)m.src[c])[from]; break;
         default: ((long long*)m.dst[c])[to] = ((const long long*)m.src[c])[from]; break;
+      }
+    }
+  }
+}
+
+// A run of a new server set: new rows [start, next run's start) are old rows prev[start].. in order, or new rows when
+// prev[start] < 0.  A run starts where the set starts, where a kept row does not follow its predecessor's old row, and
+// where kept and new rows alternate.
+struct RunHead {
+  const int* prev;
+  __device__ bool operator()(int i) const {
+    if (i == 0) return true;
+    const int a = prev[i - 1], b = prev[i];
+    return (a < 0) != (b < 0) || (b >= 0 && b != a + 1);
+  }
+};
+
+// Every column of `m`, `per` elements per row, laid out for a new set of n_rows rows: each run of *n_runs (starts[]:
+// their first new rows, ascending) copied from the old column as one contiguous range, new rows zero-filled (the nil
+// candidate, a grid level that is not ok, frontier 0).  Column blockIdx.y; a warp takes 32 * CHUNKS consecutive 16-byte
+// chunks of it at a time (16-byte loads and stores wherever source and destination are both aligned), looks up the run
+// of its first chunk and walks forward.  Memory-bound: every destination byte is written once and every kept one read
+// once, with streaming cache hints since neither side is touched again by this kernel.
+template <int CHUNKS>
+__global__ void __launch_bounds__(256) reindex_rows_kernel(RowMoves m, const int* prev, const int* starts,
+                                                           const int* n_runs, int n_rows, int per) {
+  const int c = blockIdx.y;
+  if (c >= m.n) return;
+  const int nr = *n_runs;
+  const unsigned long long rb = (unsigned long long)per * m.width[c], total = (unsigned long long)n_rows * rb;
+  const unsigned long long n_chunks = (total + 15) / 16, per_warp = 32ull * CHUNKS;
+  const int lane = threadIdx.x & 31;
+  const unsigned long long warps = (unsigned long long)gridDim.x * (blockDim.x / 32);
+  const char* src = m.src[c];
+  char* dst = m.dst[c];
+  auto run_end = [&](int r) { return (unsigned long long)(r + 1 < nr ? starts[r + 1] : n_rows) * rb; };
+  for (unsigned long long w = blockIdx.x * (unsigned long long)(blockDim.x / 32) + threadIdx.x / 32; w * per_warp < n_chunks;
+       w += warps) {
+    unsigned long long off = (w * per_warp + lane) * 16;
+    if (off >= total) continue;
+    int lo = 0, hi = nr;   // the run holding byte `off`: the last with start * rb <= off
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if ((unsigned long long)starts[mid] * rb <= off) lo = mid; else hi = mid;
+    }
+    int r = lo;
+#pragma unroll 1
+    for (int k = 0; k < CHUNKS && off < total; k++, off += 32 * 16) {
+      while (off >= run_end(r)) r++;
+      const unsigned long long end = run_end(r);
+      const int from = prev[starts[r]];
+      const unsigned long long s_off = (unsigned long long)from * rb + (off - (unsigned long long)starts[r] * rb);
+      if (off + 16 <= end && (from < 0 || (s_off & 15) == 0)) {
+        const uint4 v = from < 0 ? make_uint4(0, 0, 0, 0) : __ldcs((const uint4*)(src + s_off));
+        __stcs((uint4*)(dst + off), v);
+        continue;
+      }
+      // a chunk across a run boundary or off the source's alignment (rows of a width that is not a multiple of 16),
+      // or the column's last bytes: byte by byte
+      int rr = r;
+      for (unsigned long long b = off; b < off + 16 && b < total; b++) {
+        while (b >= run_end(rr)) rr++;
+        const int f = prev[starts[rr]];
+        dst[b] = f < 0 ? 0 : src[(unsigned long long)f * rb + (b - (unsigned long long)starts[rr] * rb)];
       }
     }
   }

@@ -6,7 +6,8 @@ entry points they replace:
     load_system      System.SetFromSpec           pkg/core/system.go:82
     calculate        System.Calculate             pkg/core/system.go:258
     update_servers   AddServerInfoToSystemData    internal/utils/utils.go:204 (loads + current allocations)
-    recalculate      System.Calculate, for the servers update_servers changed
+    recalculate      System.Calculate, for the servers update_servers / update_server_set changed
+    update_server_set  System.AddServerFromSpec / RemoveServer   pkg/core/system.go:160 (the whole server set)
     solve            Manager.Optimize             pkg/manager/manager.go:21
     candidates       Server.AllAllocations        pkg/core/server.go:138
     solution         System.GenerateSolution      pkg/core/system.go:303
@@ -95,6 +96,7 @@ def load_library():
     L.wva_calculate.argtypes = [ctxp]
     L.wva_update_servers.argtypes = [ctxp] + [C.c_void_p] * len(abi.CYCLE_ARRAYS)
     L.wva_recalculate.argtypes = [ctxp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.wva_update_server_set.argtypes = [ctxp, C.c_int32, C.c_void_p, C.POINTER(abi.System)]
     L.wva_solve.argtypes = [ctxp]
     L.wva_get_candidates.argtypes = [ctxp, C.POINTER(abi.Candidates)]
     L.wva_set_candidates.argtypes = [ctxp, C.POINTER(abi.Candidates)]
@@ -129,7 +131,7 @@ def load_library():
 
 
 EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_last_error", "wva_launch_count",
-           "wva_load_system", "wva_calculate", "wva_update_servers", "wva_recalculate", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
+           "wva_load_system", "wva_calculate", "wva_update_servers", "wva_recalculate", "wva_update_server_set", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
            "wva_analyze_grid", "wva_grid_run", "wva_grid_fetch", "wva_grid_update", "wva_mm1k_eval", "wva_saturation_v1",
            "wva_saturation_upload", "wva_saturation_run", "wva_saturation_fetch", "wva_limit", "wva_saturation_v2",
            "wva_cost_aware_optimize", "wva_enforce", "wva_pipeline_v2", "wva_host_alloc", "wva_host_free", "wva_last_timing",
@@ -266,6 +268,25 @@ class Engine:
         nr, nv = C.c_int64(), C.c_int64()
         self._check(self.lib.wva_recalculate(self.ctx, C.byref(nr), C.byref(nv)), "wva_recalculate")
         return nr.value, nv.value
+
+    def update_server_set(self, prev, sysd: dict):
+        """The loaded system's server set replaced in place by the servers of `sysd` (only its srv_* arrays and n_servers
+        are read): prev[i] = index in the loaded system of new server i, or -1 for a new one.  Resident candidates and
+        grid follow the new set; the servers that changed are re-sized by the next recalculate() and re-evaluated by the
+        next grid_update()."""
+        S2 = int(sysd["n_servers"])
+        p = np.ascontiguousarray(prev, np.int32).reshape(-1)
+        if p.size != S2:
+            raise WvaError(f"update_server_set: prev has {p.size} entries, the new set has {S2} servers")
+        st, keep = abi.make_system({**sysd, "n_acc": 0, "n_types": 0, "n_models": 0,   # the loaded tables stay
+                                    **{k: np.zeros(0, dt) for k, (dt, e) in abi.SYSTEM_ARRAYS.items() if e != "S"}})
+        keep.append(p if p.size else np.zeros(1, np.int32))
+        self._check(self.lib.wva_update_server_set(self.ctx, S2, keep[-1].ctypes.data, C.byref(st)),
+                    "wva_update_server_set")
+        self.S = S2
+        lo, hi = C.c_int32(), C.c_int32()
+        self._check(self.lib.wva_comm_shard(self.ctx, C.byref(lo), C.byref(hi)), "wva_comm_shard")
+        self.lo, self.hi = lo.value, hi.value
 
     def solve(self):
         self._check(self.lib.wva_solve(self.ctx), "wva_solve")

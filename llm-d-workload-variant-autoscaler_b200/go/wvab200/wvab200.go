@@ -114,6 +114,64 @@ func (x *Ctx) GridUpdate() (regridded int64, err error) {
 	return int64(n), err
 }
 
+// ServerColumns are the 15 server columns of a wva_system, one entry per server in ascending-name order.
+type ServerColumns struct {
+	Model, Priority, MinReplicas, MaxBatch       []int32
+	KeepAcc, TargetPresent                       []uint8
+	SLOTTFT, SLOITL, SLOTPS, Arrival             []float32
+	InTokens, OutTokens, CurAcc, CurReplicas     []int32
+	CurCost                                      []float32
+}
+
+// UpdateServerSet replaces the server set of the loaded system in place (System.AddServerFromSpec / RemoveServer for a
+// whole cycle): prev[i] is the loaded index of new server i, or -1 for a new one; cols are the new set's columns.
+// Accelerators, models and perf data stay those of the loaded system (INTEGRATION.md §3, per-cycle use).  Recalculate
+// and GridUpdate then bring the candidates and the resident grid up to date.
+func (x *Ctx) UpdateServerSet(prev []int32, cols *ServerColumns) error {
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	n := len(prev)
+	for _, l := range []int{len(cols.Model), len(cols.Priority), len(cols.MinReplicas), len(cols.MaxBatch), len(cols.KeepAcc),
+		len(cols.TargetPresent), len(cols.SLOTTFT), len(cols.SLOITL), len(cols.SLOTPS), len(cols.Arrival), len(cols.InTokens),
+		len(cols.OutTokens), len(cols.CurAcc), len(cols.CurReplicas), len(cols.CurCost)} {
+		if l != n {
+			return fmt.Errorf("UpdateServerSet: a column's length differs from len(prev)")
+		}
+	}
+	var pin runtime.Pinner // C copies the columns before returning
+	defer pin.Unpin()
+	p32 := func(s []int32) *C.int32_t {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.int32_t)(unsafe.Pointer(&s[0]))
+	}
+	pf := func(s []float32) *C.float {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.float)(unsafe.Pointer(&s[0]))
+	}
+	pu := func(s []uint8) *C.uint8_t {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.uint8_t)(unsafe.Pointer(&s[0]))
+	}
+	sys := C.wva_system{
+		n_servers: C.int32_t(n),
+		srv_model: p32(cols.Model), srv_priority: p32(cols.Priority), srv_min_replicas: p32(cols.MinReplicas),
+		srv_max_batch: p32(cols.MaxBatch), srv_keep_acc: pu(cols.KeepAcc), srv_target_present: pu(cols.TargetPresent),
+		srv_slo_ttft: pf(cols.SLOTTFT), srv_slo_itl: pf(cols.SLOITL), srv_slo_tps: pf(cols.SLOTPS), srv_arrival: pf(cols.Arrival),
+		srv_in_tokens: p32(cols.InTokens), srv_out_tokens: p32(cols.OutTokens),
+		srv_cur_acc: p32(cols.CurAcc), srv_cur_replicas: p32(cols.CurReplicas), srv_cur_cost: pf(cols.CurCost),
+	}
+	return x.err(C.wva_update_server_set(x.c, C.int32_t(n), p32(prev), &sys), "wva_update_server_set")
+}
+
 // index maps built from SORTED names: ascending index is then a valid Go map order and the
 // name-based tie-breaks of the reference become index comparisons.
 type index struct {

@@ -151,6 +151,26 @@ def differs_only_in_cycle_columns(old: dict, new: dict) -> bool:
     return True
 
 
+def server_set_prev(old_index: SpecIndex, old: dict, new_index: SpecIndex, new: dict):
+    """The `prev` map of Engine.update_server_set from the system on the device (old) to a new one, or None when the
+    two flattened specs differ in more than their servers: prev[i] = old index of new server i (by name), -1 for a new
+    server.  Every array and scalar that is not a server column (accelerators, types and capacity, models and perf
+    data, the optimizer) must be equal byte for byte; the server set and every srv_* column may change."""
+    if old.keys() != new.keys():
+        return None
+    for k, a in old.items():
+        if k.startswith("srv_") or k == "n_servers":
+            continue
+        b = new[k]
+        if isinstance(a, np.ndarray) or isinstance(b, np.ndarray):
+            a, b = np.asarray(a), np.asarray(b)
+            if a.dtype != b.dtype or a.shape != b.shape or a.tobytes() != b.tobytes():
+                return None
+        elif a != b:
+            return None
+    return np.array([old_index.server_of.get(name, -1) for name in new_index.servers], np.int32)
+
+
 def solution_to_spec(sol: dict, idx: SpecIndex, spec_servers: dict | None = None) -> dict:
     """Solution arrays -> config.AllocationSolution JSON shape (System.GenerateSolution, system.go:303-330):
     a server with no allocation is absent; the zero-load allocation has accelerator ""."""
