@@ -342,7 +342,7 @@ struct wva_ctx {
   int table_mode = 0;        // WVA_OPT_TABLE_MODE
   int greedy_mode = 0;       // WVA_OPT_GREEDY_MODE
   int grid_defer = 0;        // WVA_OPT_GRID_DEFER
-  int lane_sizer_mode = 2;   // 1 flattened, 2 lock-step (default), 3 lock-step with two chains per lane (slower: measured)
+  int lane_sizer_mode = 2;   // the sizer mode WVA_OPT_FORCE_LANE_SIZER forces while force_lane_sizer is set (launch_sizer)
   int A = 0, T = 0, M = 0, S = 0;
   uint8_t unlimited = 1, delayed = 0;
   int policy = 0;
@@ -527,66 +527,62 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
 // ------------------------------------------------------------------ calculate
 }  // extern "C" (templates need C++ linkage)
 template <int THREADS, bool SMEM>
-static cudaError_t launch_sizer(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v, int blocks, size_t smem,
+static cudaError_t launch_sizer(wva_ctx* ctx, int mode, const SysView& sys_v, const CandView& cand_v, int blocks, size_t smem,
                                 unsigned long long n_pairs, int nmax, float* gtab, int* ovf_list) {
-  // lane_sizer_mode 1 = flattened state machine (sizer_kernel.cuh); 2 = lock-step rounds; 3 = lock-step with two
-  // chains per lane; 4 = lock-step, every pair split into a TTFT item and an ITL item (mid-size systems); 5 = split
-  // items whose second chain evaluates the predicted next bisection point (wva_core.cuh spec2_*)
+  // mode 1 = flattened state machine (a burst of single chain states per round); 2 = lock-step rounds; 3 = lock-step
+  // with two chains per lane; 4 = lock-step, every pair split into a TTFT item and an ITL item (mid-size systems); 5 =
+  // split items whose second chain evaluates the predicted next bisection point (wva_core.cuh spec2_*)
   cudaError_t e;
-  if (ctx->lane_sizer_mode == 1) {
-    auto k = sizer_kernel<THREADS, SMEM>;
-    e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  SplitWs sw = {nullptr, nullptr, nullptr};
+  const bool split = mode == 4 || mode == 5;
+  if (split) {
+    Layout L;
+    e = lay_out(ctx->split_ws, L, [&](Layout& f) { f(2 * n_pairs, 0, sw.res); f(2 * n_pairs, 0, sw.solves); f(n_pairs, 0, sw.cnt); });
     if (e != cudaSuccess) return e;
-    k<<<blocks, THREADS, smem, ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, gtab, ctx->d_ctr, ovf_list);
-  } else {
-    SplitWs sw = {nullptr, nullptr, nullptr};
-    const bool split = ctx->lane_sizer_mode == 4 || ctx->lane_sizer_mode == 5;
-    if (split) {
-      Layout L;
-      e = lay_out(ctx->split_ws, L, [&](Layout& f) { f(2 * n_pairs, 0, sw.res); f(2 * n_pairs, 0, sw.solves); f(n_pairs, 0, sw.cnt); });
-      if (e != cudaSuccess) return e;
-      e = cudaMemsetAsync(sw.cnt, 0, (size_t)n_pairs * 4, ctx->stream);
-      if (e != cudaSuccess) return e;
-    }
-    // length-sorted queue: float32 probe -> (N, expected chain length) keys -> descending radix sort of the item ids
-    const unsigned* order = nullptr;
-    const unsigned long long n_items = split ? 2 * n_pairs : n_pairs;
-    // the sorted queue + gang refill pays between ~130 and ~1500 pairs per SM (the items then fill 1.5-15 waves and
-    // longest-first ordering shortens the tail); below, every lane holds one item and the probe is pure overhead; far
-    // above, the gain no longer covers the probe's variance.  With the table in global memory it is kept at any size.
-    const bool by_size = n_pairs > (unsigned long long)ctx->sm_count * 130 &&
-                         (n_pairs <= (unsigned long long)ctx->sm_count * 1500 || !SMEM);
-    const bool do_sort = ctx->length_sort < 0 ? by_size : ctx->length_sort != 0;
-    const bool do_gang = ctx->gang_refill < 0 ? by_size : ctx->gang_refill != 0;
-    if (do_sort && n_items >= 64 && n_items < (1ull << 31)) {
-      size_t tmp = 0;
-      cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr,
-                                                (unsigned*)nullptr, (int)n_items, 0, 32, ctx->stream);
-      unsigned *k_in = nullptr, *k_out = nullptr, *v_in = nullptr, *v_out = nullptr;
-      unsigned char* d_tmp = nullptr;
-      Layout L;
-      e = lay_out(ctx->order_ws, L, [&](Layout& f) {
-        f(n_items, 0, k_in); f(n_items, 0, k_out); f(n_items, 0, v_in); f(n_items, 0, v_out); f(tmp, 0, d_tmp);
-      });
-      if (e != cudaSuccess) return e;
-      const unsigned pb = (unsigned)((n_items + 127) / 128);
-      if (split) sizer_probe_kernel<true><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
-      else sizer_probe_kernel<false><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
-      e = cub::DeviceRadixSort::SortPairsDescending(d_tmp, tmp, k_in, k_out, v_in, v_out, (int)n_items, 0, 32, ctx->stream);
-      if (e != cudaSuccess) return e;
-      ctx->launches += 4;
-      order = v_out;
-    }
-    auto k = (ctx->lane_sizer_mode == 5) ? sizer_lane_kernel<THREADS, SMEM, true, true>
-           : split ? sizer_lane_kernel<THREADS, SMEM, false, true>
-           : (ctx->lane_sizer_mode == 3) ? sizer_lane_kernel<THREADS, SMEM, true, false>
-                                         : sizer_lane_kernel<THREADS, SMEM, false, false>;
-    if (THREADS == 256 && !SMEM && !split && ctx->lane_sizer_mode != 3 && ctx->lane_sizer_mode != 5)
-      k = sizer_lane_kernel_gtab_2blk;                 // the same body under a 128-register cap (2 blocks per SM)
-    e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    e = cudaMemsetAsync(sw.cnt, 0, (size_t)n_pairs * 4, ctx->stream);
     if (e != cudaSuccess) return e;
-    k<<<blocks, THREADS, smem, ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, gtab, ctx->d_ctr, ovf_list, sw, order, do_gang ? 1 : 0);
   }
+  // length-sorted queue: float32 probe -> (N, expected chain length) keys -> descending radix sort of the item ids
+  const unsigned* order = nullptr;
+  const unsigned long long n_items = split ? 2 * n_pairs : n_pairs;
+  // the sorted queue + gang refill pays between ~130 and ~1500 pairs per SM (the items then fill 1.5-15 waves and
+  // longest-first ordering shortens the tail); below, every lane holds one item and the probe is pure overhead; far
+  // above, the gain no longer covers the probe's variance.  With the table in global memory it is kept at any size.
+  // The flattened mode (1) takes neither.
+  const bool by_size = n_pairs > (unsigned long long)ctx->sm_count * 130 &&
+                       (n_pairs <= (unsigned long long)ctx->sm_count * 1500 || !SMEM);
+  const bool do_sort = mode != 1 && (ctx->length_sort < 0 ? by_size : ctx->length_sort != 0);
+  const bool do_gang = mode != 1 && (ctx->gang_refill < 0 ? by_size : ctx->gang_refill != 0);
+  if (do_sort && n_items >= 64 && n_items < (1ull << 31)) {
+    size_t tmp = 0;
+    cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr,
+                                              (unsigned*)nullptr, (int)n_items, 0, 32, ctx->stream);
+    unsigned *k_in = nullptr, *k_out = nullptr, *v_in = nullptr, *v_out = nullptr;
+    unsigned char* d_tmp = nullptr;
+    Layout L;
+    e = lay_out(ctx->order_ws, L, [&](Layout& f) {
+      f(n_items, 0, k_in); f(n_items, 0, k_out); f(n_items, 0, v_in); f(n_items, 0, v_out); f(tmp, 0, d_tmp);
+    });
+    if (e != cudaSuccess) return e;
+    const unsigned pb = (unsigned)((n_items + 127) / 128);
+    if (split) sizer_probe_kernel<true><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
+    else sizer_probe_kernel<false><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
+    e = cub::DeviceRadixSort::SortPairsDescending(d_tmp, tmp, k_in, k_out, v_in, v_out, (int)n_items, 0, 32, ctx->stream);
+    if (e != cudaSuccess) return e;
+    ctx->launches += 4;
+    order = v_out;
+  }
+  // <THREADS, SMEM, DUAL, SPLIT, FLAT>; mode 2 with its table in global memory runs the same body under a 128-register
+  // cap (2 blocks per SM)
+  auto k = mode == 1 ? sizer_lane_kernel<THREADS, SMEM, false, false, true>
+         : mode == 3 ? sizer_lane_kernel<THREADS, SMEM, true, false, false>
+         : mode == 4 ? sizer_lane_kernel<THREADS, SMEM, false, true, false>
+         : mode == 5 ? sizer_lane_kernel<THREADS, SMEM, true, true, false>
+         : THREADS == 256 && !SMEM ? sizer_lane_kernel_gtab_2blk
+                                   : sizer_lane_kernel<THREADS, SMEM, false, false, false>;
+  e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  k<<<blocks, THREADS, smem, ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, gtab, ctx->d_ctr, ovf_list, sw, order, do_gang ? 1 : 0);
   ctx->launches++;
   return cudaGetLastError();
 }
@@ -657,33 +653,21 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
     if (nmax < 1) nmax = 1;
     const int NLIMIT = 1 << 16;
     if (nmax > NLIMIT) nmax = NLIMIT;  // pairs beyond it are flagged through limit_hit
-    // 2) pick geometry: the head table (4 B x nmax per lane) lives in shared memory when at
-    //    least 64 lanes fit on an SM; lanes per SM are maximised over CTA sizes {256,192,128,64}
-    //    (1 KB per CTA is reserved by the driver).  Otherwise the table goes to global memory.
     const size_t SMEM_PER_SM = 224 * 1024;
-    const size_t per_lane = (size_t)nmax * 4;
-    const int sizes[4] = {256, 192, 128, 64};
-    int best_threads = 0, best_per_sm = 0;
-    for (int i = 0; i < 4; i++) {
-      size_t cta = per_lane * sizes[i] + 1024;
-      int per_sm = (int)(SMEM_PER_SM / cta);
-      if (per_sm * sizes[i] > 1024) per_sm = 1024 / sizes[i];
-      if (per_sm * sizes[i] > best_threads * best_per_sm) { best_threads = sizes[i]; best_per_sm = per_sm; }
-    }
-    // small problems are latency bound: spread the pairs over every SM with as few lanes per SM
-    // as needed instead of filling the first SMs (lanes pull one pair each from the queue)
-    // mid-size systems (measured: up to ~200 pairs per SM) still leave lanes idle: split every pair into a
-    // TTFT item and an ITL item, which halves the chain of dependent solves per work item
-    // crossovers (natural queue order): split items up to ~180 pairs per SM, split items with a speculative second
+    // 2) the lane sizer's mode, unless forced.  Mid-size systems (measured: up to ~200 pairs per SM) leave lanes idle:
+    // split every pair into a TTFT item and an ITL item, which halves the chain of dependent solves per work item.
+    // Crossovers (natural queue order): split items up to ~180 pairs per SM, split items with a speculative second
     // chain (mode 5) up to ~380, whole pairs (mode 2, the searches share evaluations) beyond
-    if (!ctx->force_lane_sizer)
-      ctx->lane_sizer_mode = (n_pairs <= (unsigned long long)ctx->sm_count * 180) ? 4
-                           : (n_pairs <= (unsigned long long)ctx->sm_count * 380) ? 5 : 2;
-    // large systems: the pool sizer (sizer_pool_kernel.cuh) regroups the pending solves of 1024 pairs per SM by
-    // length every time a warp goes back for work (88-92 % live lane-steps instead of 49-62 %); it overtakes the lane
-    // sizer from ~640 pairs per SM
+    const int mode = ctx->force_lane_sizer ? ctx->lane_sizer_mode
+                   : (n_pairs <= (unsigned long long)ctx->sm_count * 180) ? 4
+                   : (n_pairs <= (unsigned long long)ctx->sm_count * 380) ? 5 : 2;
+    // 3) the sizer.  Large systems: the pool sizer (sizer_pool_kernel.cuh) regroups the pending solves of 1024 pairs
+    // per SM by length every time a warp goes back for work (88-92 % live lane-steps instead of 49-62 %); it overtakes
+    // the lane sizer from ~640 pairs per SM
     const bool pool_auto = !ctx->force_lane_sizer && n_pairs > (unsigned long long)ctx->sm_count * 640 && nmax <= 4096;
-    if (pool_auto || (ctx->force_lane_sizer && ctx->lane_sizer_mode == 6)) {
+    const size_t warp_tab = (size_t)nmax * 20;
+    cudaError_t e = cudaSuccess;
+    if (pool_auto || (ctx->force_lane_sizer && mode == 6)) {
       const int P = POOL_PMAX;
       const size_t pool_bytes = (size_t)ctx->sm_count * P * sizeof(PoolEntry);
       CK(ctx->pool_ws.reserve(pool_bytes + 512));
@@ -695,54 +679,62 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
       cudaError_t pe = cudaGetLastError();
       if (pe != cudaSuccess) { ctx->last_error = std::string("pool sizer launch: ") + cudaGetErrorString(pe); return WVA_ERR_CUDA; }
       ctx->timing.sizer_kernel = 4;
-      goto sizer_done;
-    }
-    const unsigned long long n_items = (ctx->lane_sizer_mode >= 4) ? 2 * n_pairs : n_pairs;
-    const unsigned long long lanes_needed = (n_items + ctx->sm_count - 1) / ctx->sm_count;
-    if (best_per_sm >= 1 && lanes_needed <= 256 && lanes_needed < (unsigned long long)best_threads * best_per_sm) {
-      int t = 64;
-      while ((unsigned long long)t < lanes_needed) t += 64;
-      if (per_lane * t + 1024 <= SMEM_PER_SM) { best_threads = t; best_per_sm = 1; }
-    }
-    cudaError_t e;
-    // Small / medium systems are bound by the critical path of their slowest pair: use the
-    // warp-per-pair sizer (speculative bisection, sizer_warp_kernel.cuh) while the system is small
-    // (measured crossover against the lock-step lane sizer: ~32 pairs per SM) and its per-warp
-    // tables (20 B x nmax) fit in shared memory.
-    const size_t warp_tab = (size_t)nmax * 20;
-    if (n_pairs <= (unsigned long long)ctx->sm_count * 32 && warp_tab * 4 + 1024 <= SMEM_PER_SM && !ctx->force_lane_sizer) {
+    } else if (n_pairs <= (unsigned long long)ctx->sm_count * 32 && warp_tab * 4 + 1024 <= SMEM_PER_SM && !ctx->force_lane_sizer) {
+      // Small / medium systems are bound by the critical path of their slowest pair: the warp-per-pair sizer
+      // (speculative bisection, sizer_warp_kernel.cuh) while the system is small (measured crossover against the
+      // lock-step lane sizer: ~32 pairs per SM) and its per-warp tables (20 B x nmax) fit in shared memory.
+      ctx->timing.sizer_kernel = 1;
       if (warp_tab * 8 <= 48 * 1024) {
         int per_sm = (int)(SMEM_PER_SM / (warp_tab * 8 + 1024)); if (per_sm > 6) per_sm = 6; if (per_sm < 1) per_sm = 1;
         e = launch_sizer_warp<8>(ctx, sys_v, cand_v, ctx->sm_count * per_sm, warp_tab * 8, n_pairs, nmax, d_ovf);
-        ctx->timing.sizer_kernel = 1;
       } else {
         int per_sm = (int)(SMEM_PER_SM / (warp_tab * 4 + 1024)); if (per_sm > 8) per_sm = 8; if (per_sm < 1) per_sm = 1;
         e = launch_sizer_warp<4>(ctx, sys_v, cand_v, ctx->sm_count * per_sm, warp_tab * 4, n_pairs, nmax, d_ovf);
-        ctx->timing.sizer_kernel = 1;
-      }
-    } else
-    // Head table placement: N = 256 leaves 192 lanes per SM in shared memory (1.5 warps per scheduler), slower than the
-    // table in global memory / L2 with two 256-thread blocks per SM under a 128-register cap; at N = 128 (384 lanes in
-    // shared memory) and N = 64 shared memory wins.
-    if (best_per_sm >= 1 && ctx->table_mode != 2 && (ctx->table_mode == 1 || best_threads * best_per_sm > 256 || n_pairs <= (unsigned long long)ctx->sm_count * 512)) {
-      int blocks = ctx->sm_count * best_per_sm;
-      size_t smem = per_lane * best_threads;
-      ctx->timing.sizer_kernel = 2;
-      switch (best_threads) {
-        case 256: e = launch_sizer<256, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-        case 192: e = launch_sizer<192, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-        case 128: e = launch_sizer<128, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-        default: e = launch_sizer<64, true>(ctx, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
       }
     } else {
-      int blk = ctx->sm_count * 2;
-      ctx->timing.sizer_kernel = 3;
-      CK(ctx->gtab.reserve((size_t)blk * 256 * per_lane));
-      e = launch_sizer<256, false>(ctx, sys_v, cand_v, blk, 0, n_pairs, nmax, (float*)ctx->gtab.p, d_ovf);
+      // The lane sizer.  Its head table (4 B x nmax per lane) lives in shared memory when at least 64 lanes fit on an
+      // SM; lanes per SM are maximised over CTA sizes {256,192,128,64} (1 KB per CTA is reserved by the driver).
+      // Otherwise the table goes to global memory.
+      const size_t per_lane = (size_t)nmax * 4;
+      const int sizes[4] = {256, 192, 128, 64};
+      int best_threads = 0, best_per_sm = 0;
+      for (int i = 0; i < 4; i++) {
+        size_t cta = per_lane * sizes[i] + 1024;
+        int per_sm = (int)(SMEM_PER_SM / cta);
+        if (per_sm * sizes[i] > 1024) per_sm = 1024 / sizes[i];
+        if (per_sm * sizes[i] > best_threads * best_per_sm) { best_threads = sizes[i]; best_per_sm = per_sm; }
+      }
+      // small problems are latency bound: spread the items over every SM with as few lanes per SM as needed instead
+      // of filling the first SMs (lanes pull one item each from the queue)
+      const unsigned long long n_items = (mode >= 4) ? 2 * n_pairs : n_pairs;
+      const unsigned long long lanes_needed = (n_items + ctx->sm_count - 1) / ctx->sm_count;
+      if (best_per_sm >= 1 && lanes_needed <= 256 && lanes_needed < (unsigned long long)best_threads * best_per_sm) {
+        int t = 64;
+        while ((unsigned long long)t < lanes_needed) t += 64;
+        if (per_lane * t + 1024 <= SMEM_PER_SM) { best_threads = t; best_per_sm = 1; }
+      }
+      // Head table placement: N = 256 leaves 192 lanes per SM in shared memory (1.5 warps per scheduler), slower than
+      // the table in global memory / L2 with two 256-thread blocks per SM under a 128-register cap; at N = 128 (384
+      // lanes in shared memory) and N = 64 shared memory wins.
+      if (best_per_sm >= 1 && ctx->table_mode != 2 && (ctx->table_mode == 1 || best_threads * best_per_sm > 256 || n_pairs <= (unsigned long long)ctx->sm_count * 512)) {
+        int blocks = ctx->sm_count * best_per_sm;
+        size_t smem = per_lane * best_threads;
+        ctx->timing.sizer_kernel = 2;
+        switch (best_threads) {
+          case 256: e = launch_sizer<256, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          case 192: e = launch_sizer<192, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          case 128: e = launch_sizer<128, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          default: e = launch_sizer<64, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+        }
+      } else {
+        int blk = ctx->sm_count * 2;
+        ctx->timing.sizer_kernel = 3;
+        CK(ctx->gtab.reserve((size_t)blk * 256 * per_lane));
+        e = launch_sizer<256, false>(ctx, mode, sys_v, cand_v, blk, 0, n_pairs, nmax, (float*)ctx->gtab.p, d_ovf);
+      }
     }
     if (e != cudaSuccess) { ctx->last_error = std::string("sizer launch: ") + cudaGetErrorString(e); return WVA_ERR_CUDA; }
   }
-sizer_done:
   CK(cudaEventRecord(ctx->ev[3], ctx->stream));
   SizerCounters hc;
   CK(cudaMemcpyAsync(&hc, ctx->d_ctr, sizeof(hc), cudaMemcpyDeviceToHost, ctx->stream));

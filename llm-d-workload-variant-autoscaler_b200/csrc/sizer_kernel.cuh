@@ -1,12 +1,6 @@
-// sizer_kernel.cuh — System.Calculate on the device: one lane per (server,
-// accelerator) candidate, persistent CTAs pulling pairs from a global counter.
-//
-// SIMT shape: the inner loop body is ONE birth-death state of whatever solve the
-// lane is in (pass 1 or pass 2 of any bisection step of any pair), so lanes of a
-// warp never wait for each other's solve lengths; only the rare transitions
-// (solve finished -> bisection bookkeeping, pair finished -> fetch + BuildModel)
-// diverge.  The head table mu_n (float32) of each lane lives in shared memory,
-// column-interleaved ([n][thread]) so a lane always hits bank (tid % 32).
+// sizer_kernel.cuh — what the sizer kernels (lane, warp, pool and the overflow slow path) share: the
+// counters, the retirement of a float64-overflowing pair, the max-batch reduction that decides the
+// head-table geometry, and the warp broadcast of one lane's pair model for cooperative BuildModel.
 #pragma once
 #include "wva_core.cuh"
 
@@ -56,86 +50,19 @@ __global__ void __launch_bounds__(256) max_batch_kernel(SysView s, unsigned long
   if ((threadIdx.x & 31) == 0 && best > 0) atomicMax(out, best);
 }
 
-template <int THREADS, bool SMEM_TABLE>
-__global__ void __launch_bounds__(THREADS)
-sizer_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
-             SizerCounters* ctr, int* overflow_list) {
-  extern __shared__ float smem_tab[];
-  const int lane = threadIdx.x & 31;
+// Lane `src`'s service-rate coefficients (the fields rate_coef reads) and N, on every lane of the warp.
+__device__ __forceinline__ PairModel shfl_model(const PairModel& m, int src) {
   const unsigned full = 0xffffffffu;
-  float* tab;
-  int stride;
-  if (SMEM_TABLE) { tab = smem_tab + threadIdx.x; stride = THREADS; }
-  else { tab = gtab + ((size_t)blockIdx.x * THREADS + threadIdx.x); stride = gridDim.x * THREADS; }
-
-  SizerLane z;
-  SolveStats st;
-  bool live = false, exhausted = false;
-  unsigned long long my_solves = 0, my_states = 0;
-
-  while (true) {
-    // ---- refill: lanes without work fetch pairs until one needs sizing -----------------
-    bool need_table = false;
-    if (!live && !exhausted) {
-      while (true) {
-        unsigned long long pair = atomicAdd(&ctr->next_pair, 1ull);
-        if (pair >= n_pairs) { exhausted = true; break; }
-        int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
-        int lim = 0;
-        int rc = sizer_setup(z, s, out, srv, acc, nmax, &lim);
-        if (lim) ctr->limit_hit = 1;
-        if (rc == SETUP_NEEDS_TABLE) { need_table = true; break; }
-      }
-    }
-    // ---- BuildModel, cooperatively: the warp fills each requesting lane's column --------
-    unsigned need = __ballot_sync(full, need_table);
-    while (need) {
-      int src = __ffs(need) - 1;
-      need &= need - 1;
-      PairModel b;
-      b.alpha = __shfl_sync(full, z.m.alpha, src);
-      b.beta = __shfl_sync(full, z.m.beta, src);
-      b.in_tok = __shfl_sync(full, z.m.in_tok, src);
-      b.out_tok = __shfl_sync(full, z.m.out_tok, src);
-      b.slope = __shfl_sync(full, z.m.slope, src);
-      b.pre_c = __shfl_sync(full, z.m.pre_c, src);
-      b.dec_c = __shfl_sync(full, z.m.dec_c, src);
-      b.N = __shfl_sync(full, z.m.N, src);
-      // column of lane `src` is this lane's column shifted by (src - lane)
-      model_fill_table(b, tab + (src - lane), stride, lane, 32);
-    }
-    __syncwarp();
-    if (need_table) {
-      model_finish(z.m, tab, stride);
-      live = sizer_begin(z, s, out);
-      if (!live) { my_solves += z.solves; }
-    }
-    if (!__any_sync(full, live || !exhausted)) break;
-
-    // ---- steady state: advance every live lane by a burst of states ----------------------
-    // (a burst bounds how often the warp re-converges for refills)
-    for (int it = 0; it < 64; it++) {
-      if (live) {
-        if (chain_step(z.c, z.m, st)) {
-          if (z.c.phase == CH_OVERFLOW) {
-            retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
-            live = false;
-          } else {
-            live = sizer_on_solve(z, s, out, st);
-          }
-          if (!live) { my_solves += z.solves; my_states += z.states; }
-        }
-      }
-      // every 8 states: stop when the warp is idle or some lane can refill (warp-uniform)
-      if ((it & 7) == 7 && (!__any_sync(full, live) || __any_sync(full, !live && !exhausted))) break;
-    }
-  }
-  // ---- counters -----------------------------------------------------------------------------
-  for (int o = 16; o; o >>= 1) {
-    my_solves += __shfl_down_sync(full, my_solves, o);
-    my_states += __shfl_down_sync(full, my_states, o);
-  }
-  if (lane == 0) { atomicAdd(&ctr->solves, my_solves); atomicAdd(&ctr->states, my_states); }
+  PairModel b;
+  b.alpha = __shfl_sync(full, m.alpha, src);
+  b.beta = __shfl_sync(full, m.beta, src);
+  b.in_tok = __shfl_sync(full, m.in_tok, src);
+  b.out_tok = __shfl_sync(full, m.out_tok, src);
+  b.slope = __shfl_sync(full, m.slope, src);
+  b.pre_c = __shfl_sync(full, m.pre_c, src);
+  b.dec_c = __shfl_sync(full, m.dec_c, src);
+  b.N = __shfl_sync(full, m.N, src);
+  return b;
 }
 
 }  // namespace wva

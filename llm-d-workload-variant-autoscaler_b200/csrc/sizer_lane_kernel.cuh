@@ -5,7 +5,7 @@
 // arrival rate.  Between solves every lane advances its own bisection / Size / Analyze
 // state machine (wva_core.cuh sizer_on_solve), idle lanes refill from the queue.
 //
-// Compared with sizer_kernel.cuh (one state per loop iteration, lanes in arbitrary
+// Compared with the flattened round (FLAT: a burst of single states, lanes in arbitrary
 // phases) the lock-step rounds waste lanes whose chain ends early, but run ~10 instead
 // of ~70 instructions per state.  Lanes of a warp must share N for the lock-step loops
 // to be uniform; a round with mixed N falls back to the per-lane state machine.
@@ -42,10 +42,15 @@ __device__ __forceinline__ bool split_publish(SizerLane& z, const SysView& s, co
   return DUAL ? spec2_after_search(z, s, out) : sizer_after_search(z, s, out);   // -> the two Analyze solves
 }
 
-template <int THREADS, bool SMEM_TABLE, bool DUAL, bool SPLIT>
+// FLAT (WVA_OPT_FORCE_LANE_SIZER 1): a round advances every live lane by a burst of single chain_step states, each
+// lane in whatever solve it is in, so lanes never wait for each other's chain lengths; the burst bounds how often the
+// warp re-converges for refills.  It runs whole pairs in queue order (launch_sizer passes no order and no gang), and
+// its rounds are not counted in lockstep_slots.
+template <int THREADS, bool SMEM_TABLE, bool DUAL, bool SPLIT, bool FLAT>
 __device__ __forceinline__ void
 sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
                   SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {
+  static_assert(!FLAT || (!DUAL && !SPLIT), "the flattened round runs whole pairs, one chain per lane");
   extern __shared__ float smem_tab[];
   const int lane = threadIdx.x & 31;
   const unsigned full = 0xffffffffu;
@@ -80,20 +85,13 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
         if (rc == SETUP_NEEDS_TABLE) { need_table = true; if (SPLIT) z.split = (int)(item & 1); break; }
       }
     }
+    // ---- BuildModel, cooperatively: the warp fills each requesting lane's column ----------------
     unsigned need = __ballot_sync(full, need_table);
-    while (need) {   // BuildModel, cooperatively (see sizer_kernel.cuh)
+    while (need) {
       int src = __ffs(need) - 1;
       need &= need - 1;
-      PairModel b;
-      b.alpha = __shfl_sync(full, z.m.alpha, src);
-      b.beta = __shfl_sync(full, z.m.beta, src);
-      b.in_tok = __shfl_sync(full, z.m.in_tok, src);
-      b.out_tok = __shfl_sync(full, z.m.out_tok, src);
-      b.slope = __shfl_sync(full, z.m.slope, src);
-      b.pre_c = __shfl_sync(full, z.m.pre_c, src);
-      b.dec_c = __shfl_sync(full, z.m.dec_c, src);
-      b.N = __shfl_sync(full, z.m.N, src);
-      model_fill_table(b, tab + (src - lane), stride, lane, 32);
+      // column of lane `src` is this lane's column shifted by (src - lane)
+      model_fill_table(shfl_model(z.m, src), tab + (src - lane), stride, lane, 32);
     }
     __syncwarp();
     if (need_table) {
@@ -105,6 +103,23 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
     const unsigned live_mask = __ballot_sync(full, live);
     if (!live_mask) {
       if (!__any_sync(full, !exhausted)) break;
+      continue;
+    }
+    // ---- FLAT: a burst of up to 64 states per live lane ------------------------------------------
+    if (FLAT) {
+      for (int it = 0; it < 64; it++) {
+        if (live && chain_step(z.c, z.m, st)) {
+          if (z.c.phase == CH_OVERFLOW) {
+            retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
+            live = false;
+          } else {
+            live = sizer_on_solve(z, s, out, st);
+          }
+          if (!live) { my_solves += z.solves; my_states += z.states; }
+        }
+        // every 8 states: stop when the warp is idle or some lane can refill (warp-uniform)
+        if ((it & 7) == 7 && (!__any_sync(full, live) || __any_sync(full, !live && !exhausted))) break;
+      }
       continue;
     }
     // ---- one round: every live lane solves its chain at z.cur_x -------------------------------
@@ -160,14 +175,17 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
     my_solves += __shfl_down_sync(full, my_solves, o);
     my_states += __shfl_down_sync(full, my_states, o);
   }
-  if (lane == 0) { atomicAdd(&ctr->solves, my_solves); atomicAdd(&ctr->states, my_states); atomicAdd(&ctr->lockstep_slots, my_slots); }
+  if (lane == 0) {
+    atomicAdd(&ctr->solves, my_solves); atomicAdd(&ctr->states, my_states);
+    if (!FLAT) atomicAdd(&ctr->lockstep_slots, my_slots);
+  }
 }
 
-template <int THREADS, bool SMEM_TABLE, bool DUAL, bool SPLIT>
+template <int THREADS, bool SMEM_TABLE, bool DUAL, bool SPLIT, bool FLAT>
 __global__ void __launch_bounds__(THREADS)
 sizer_lane_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
                   SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {
-  sizer_lane_body<THREADS, SMEM_TABLE, DUAL, SPLIT>(s, out, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
+  sizer_lane_body<THREADS, SMEM_TABLE, DUAL, SPLIT, FLAT>(s, out, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
 }
 
 // The plain lane kernel with its table in global memory — large N on large systems (BASELINE config 3) — is launched
@@ -177,7 +195,7 @@ sizer_lane_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
 __global__ void __launch_bounds__(256, 2)
 sizer_lane_kernel_gtab_2blk(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
                             SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {
-  sizer_lane_body<256, false, false, false>(s, out, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
+  sizer_lane_body<256, false, false, false, false>(s, out, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
 }
 
 }  // namespace wva

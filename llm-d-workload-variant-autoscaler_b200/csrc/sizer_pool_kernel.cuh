@@ -289,15 +289,7 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       while (need) {
         const int src = __ffs(need) - 1;
         need &= need - 1;
-        PairModel b;
-        b.alpha = __shfl_sync(full, z.m.alpha, src);
-        b.beta = __shfl_sync(full, z.m.beta, src);
-        b.in_tok = __shfl_sync(full, z.m.in_tok, src);
-        b.out_tok = __shfl_sync(full, z.m.out_tok, src);
-        b.slope = __shfl_sync(full, z.m.slope, src);
-        b.pre_c = __shfl_sync(full, z.m.pre_c, src);
-        b.dec_c = __shfl_sync(full, z.m.dec_c, src);
-        b.N = __shfl_sync(full, z.m.N, src);
+        const PairModel b = shfl_model(z.m, src);
         float cur = 0.0f, carry = 0.0f, first = 0.0f;
         int desc = 0;
         bool e1 = true;

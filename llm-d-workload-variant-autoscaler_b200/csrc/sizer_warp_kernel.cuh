@@ -2,7 +2,7 @@
 // (server, accelerator) candidate, bisection evaluated speculatively across the lanes.
 //
 // The float32 bisection of the reference (pkg/analyzer/utils.go:26-70) is a chain of
-// ~25 dependent chain solves per target; with one lane per pair (sizer_kernel.cuh) the
+// ~25 dependent chain solves per target; with one lane per pair (sizer_lane_kernel.cuh) the
 // wall time of a small system is the critical path of its slowest pair.  Here the lanes
 // of a warp evaluate, in one round, every node of the next D levels of the bisection
 // tree (the midpoints are pure float32 arithmetic on (lo, hi), so all 2^D - 1 are known
