@@ -272,7 +272,9 @@ int32_t wva_update_servers(wva_ctx* ctx, const float* srv_arrival, const int32_t
                            const float* srv_cur_cost);
 /* Bring the candidates up to date with every wva_update_servers since the last wva_calculate / wva_recalculate:
  * re-size the servers whose sizing inputs changed (the sizer wva_calculate would pick for that many servers, on a
- * gathered copy of their columns) and re-value the ones whose current allocation alone changed.  The candidates are
+ * gathered copy of their columns) and re-value the ones whose current allocation alone changed.  With table marks of
+ * wva_update_tables pending, the pairs of the re-size-marked servers and the table-marked pairs are re-sized in place
+ * instead (the sizer picked for that many pairs), after the re-valuation; the counts stay whole servers.  The candidates are
  * bit-equal to those of a wva_calculate, except n_solves, which counts the solves of the sizer that last sized the pair
  * (the sizers spend different numbers of solves on the same result).  *n_resized / *n_revalued (either may be NULL) get the two counts of the ctx's
  * block.  WVA_ERR_STATE unless the resident candidates come from wva_calculate / wva_recalculate on the loaded system:
@@ -303,6 +305,31 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued);
  * move, so the call needs the old and the new arenas at once: about twice the grid's size with full outputs (2 x 14 GB
  * for 100 000 servers x 32 accelerators at R = 256).  Timing: h2d_ms covers the whole call. */
 int32_t wva_update_server_set(wva_ctx* ctx, int32_t n_servers, const int32_t* prev /* [S'] */, const wva_system* servers);
+/* Replace the accelerator and model performance tables of the loaded system in place: the accelerator costs an
+ * operator edits (internal/utils/utils.go:140-156) and the ModelAcceleratorPerfData a tuner re-estimates every cycle
+ * (internal/engines/analyzers/queueingmodel/tuner/tuner.go:189-244).  `tables` carries acc_cost, acc_multiplicity,
+ * acc_type ([A]) and the seven perf_* arrays ([M*A]); n_acc, n_types and n_models must be the loaded ones (adding or
+ * removing accelerators, types or models is wva_load_system).  Its server columns, type_count (wva_set_capacity) and
+ * optimizer fields are ignored.  WVA_ERR_ARG, with nothing changed, on a NULL array, another shape, or a violation of
+ * wva_load_system's table checks (acc_type in [0, T), finite alpha / beta / gamma >= 0 on every present perf row).
+ * WVA_ERR_STATE before wva_load_system.
+ * One H2D copy, then one device pass compares every entry bitwise with the resident one (-0.0 vs 0.0 is a change),
+ * writes it over it and marks table rows, not servers, so the marks stay valid across wva_update_server_set:
+ *   - a perf row (m, a) for sizing when alpha, beta, gamma, max_batch, at_tokens, acc_count or present changed, and for
+ *     the grid when any of them but acc_count changed (the grid reads neither acc_count nor acc_cost);
+ *   - an accelerator a for sizing when acc_cost[a] changed (every candidate's cost and value on it);
+ *   - nothing for acc_multiplicity and acc_type: only the allocators read them, and the solution is void until
+ *     wva_solve.
+ * Pair (s, a) of the ctx's block then needs re-sizing when srv_model[s] = m >= 0 and row (m, a) or accelerator a is
+ * sizing-marked, and re-gridding when row (m, a) is grid-marked; unknown-model servers read no table.  *n_marked (may be
+ * NULL) = the pairs of the block this call's diff marks for re-sizing.  The marks accumulate from call to call:
+ * wva_recalculate consumes the sizing marks and wva_grid_update the grid marks, each re-sizing / re-gridding every pair
+ * of a server-marked server and the table-marked pairs of the others, in place through a list of pairs, to the
+ * candidates and grid of wva_load_system + wva_calculate (+ wva_grid_run) on the updated system.  wva_calculate voids
+ * the sizing marks, wva_grid_run the grid marks, wva_load_system both; each call leaves the other kind alone.  With a
+ * communicator every rank passes the same tables and marks its own block; no collective is involved.  Timing: h2d_ms
+ * covers the whole call. */
+int32_t wva_update_tables(wva_ctx* ctx, const wva_system* tables, int64_t* n_marked);
 /* Manager.Optimize (pkg/manager/manager.go:21-27): Optimizer.Optimize
  * (pkg/solver/optimizer.go:24-36) -> Solver.Solve (solver.go:32-60) — SolveUnlimited
  * (solver.go:63-79) or SolveGreedy (greedy.go:35-105) — then AllocateByType. */
@@ -354,7 +381,9 @@ int32_t wva_grid_fetch(wva_ctx* ctx, uint8_t* ok, float* ttft, float* itl,
  * capacity of a run on the whole block.  WVA_ERR_STATE unless the resident grid comes from wva_grid_run /
  * wva_grid_update on the loaded system: before wva_load_system, after it until the next wva_grid_run, and after a
  * failed grid call.  grid_ms covers the whole call; chain_solves, chain_states, overflow_pairs and certify_fallbacks
- * are those of the re-evaluated servers, 0 when none. */
+ * are those of the re-evaluated servers, 0 when none.  With grid marks of wva_update_tables pending, every pair of a
+ * marked server and the pairs whose perf row changed are re-evaluated in place through a list of pairs, from which the
+ * deferred pass and the batch size limit are then decided; *n_regridded still counts the marked servers. */
 int32_t wva_grid_update(wva_ctx* ctx, int64_t* n_regridded);
 
 /*

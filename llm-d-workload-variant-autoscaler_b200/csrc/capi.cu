@@ -74,14 +74,16 @@ struct Ext { size_t A = 0, T = 0, M = 0, S = 0, V = 0, P = 0, R = 0, N = 0; };  
 enum { COL_OPT = 1,       // input the caller may leave NULL: its view is NULL too
        COL_DETAIL = 2,    // V1 saturation analysis field: written only by a detail run
        COL_CYCLE = 4,     // server column wva_update_servers replaces in place (ServerLoadSpec and CurrentAlloc)
-       COL_SRV = 8 };     // server column ([S]): wva_update_server_set replaces the set of them
+       COL_SRV = 8,       // server column ([S]): wva_update_server_set replaces the set of them
+       COL_TAB = 16 };    // accelerator or perf table column: wva_update_tables replaces them in place
 #define SRV_CYCLE (COL_SRV | COL_CYCLE)
 
 // The model tables come first and the server columns last: a new server set keeps the arena's prefix as it is.
 #define SYS_COLS(X)                                                                                                    \
-  X(acc_cost, n.A, 0) X(acc_multiplicity, n.A, 0) X(acc_type, n.A, 0) X(type_count, n.T, 0)                            \
-  X(perf_alpha, n.M * n.A, 0) X(perf_beta, n.M * n.A, 0) X(perf_gamma, n.M * n.A, 0) X(perf_max_batch, n.M * n.A, 0)  \
-  X(perf_at_tokens, n.M * n.A, 0) X(perf_acc_count, n.M * n.A, 0) X(perf_present, n.M * n.A, 0)                        \
+  X(acc_cost, n.A, COL_TAB) X(acc_multiplicity, n.A, COL_TAB) X(acc_type, n.A, COL_TAB) X(type_count, n.T, 0)          \
+  X(perf_alpha, n.M * n.A, COL_TAB) X(perf_beta, n.M * n.A, COL_TAB) X(perf_gamma, n.M * n.A, COL_TAB)                 \
+  X(perf_max_batch, n.M * n.A, COL_TAB) X(perf_at_tokens, n.M * n.A, COL_TAB) X(perf_acc_count, n.M * n.A, COL_TAB)    \
+  X(perf_present, n.M * n.A, COL_TAB)                                                                                  \
   X(srv_model, n.S, COL_SRV) X(srv_priority, n.S, COL_SRV) X(srv_min_replicas, n.S, COL_SRV)                           \
   X(srv_max_batch, n.S, COL_SRV) X(srv_keep_acc, n.S, COL_SRV) X(srv_target_present, n.S, COL_SRV)                     \
   X(srv_slo_ttft, n.S, COL_SRV) X(srv_slo_itl, n.S, COL_SRV) X(srv_slo_tps, n.S, COL_SRV)                              \
@@ -235,6 +237,35 @@ template <class F, class... Structs> static void each_server(size_t S, F&& f, St
   each_srv<COL_SRV>(S, f, s...);
 }
 
+// visits the accelerator and perf table columns of A accelerators and M models (not type_count: wva_set_capacity's)
+template <class F, class... Structs> static void each_table(size_t A, size_t M, F&& f, Structs&&... s) {
+  Ext n;
+  n.A = A; n.M = M;
+  each_sys(n, [&](size_t c, int flags, auto&&... col) { if (flags & COL_TAB) f(c, flags, col...); }, s...);
+}
+
+// The preconditions of the table columns, shared by wva_load_system and wva_update_tables: every array non-NULL,
+// acc_type in [0, T), and the service coefficients of every present perf row finite and >= 0.  Returns the violated
+// rule, or nullptr.
+static const char* check_table_columns(const wva_system& s, size_t A, size_t T, size_t M) {
+  Missing miss;
+  SysView none = {};
+  each_table(A, M, miss, none, s);
+  if (miss.any) return "a required array is NULL";
+  for (size_t a = 0; a < A; a++)
+    if (s.acc_type[a] < 0 || s.acc_type[a] >= (int)T) return "acc_type out of range";
+  // ServiceParms (pkg/analyzer/queueanalyzer.go:33-38) are measured service-time coefficients: finite and >= 0.  A
+  // negative or NaN coefficient makes arrival rates negative (QueueModel.Solve's gate, queuemodel.go:31) or NaN and
+  // the sizing meaningless; it is rejected here instead of being carried into the kernels.
+  for (size_t i = 0; i < M * A; i++) {
+    if (!s.perf_present[i]) continue;
+    const float a = s.perf_alpha[i], b = s.perf_beta[i], g = s.perf_gamma[i];
+    if (!(a >= 0.0f && b >= 0.0f && g >= 0.0f) || a > 3.0e38f || b > 3.0e38f || g > 3.0e38f)
+      return "perf_alpha / perf_beta / perf_gamma must be finite and >= 0";
+  }
+  return nullptr;
+}
+
 // The preconditions of the per-cycle columns, shared by wva_load_system and wva_update_servers: every array non-NULL
 // and srv_cur_acc an accelerator index or a WVA_CUR_ACC_* sentinel.  Returns the violated rule, or nullptr.
 static const char* check_cycle_columns(const wva_system& s, size_t S, int A) {
@@ -336,6 +367,8 @@ struct wva_ctx {
   bool sized = false;               // the resident candidates come from wva_calculate / wva_recalculate on this ctx
   bool marked = false;              // `marks` holds the marks of a wva_update_servers since then (else all clear)
   bool grid_marked = false;         // `grid_marks` holds the load changes since the last wva_grid_run / wva_grid_update
+  bool table_marked = false;        // tmarks.size_* hold the table changes since the last wva_calculate / wva_recalculate
+  bool table_grid_marked = false;   // tmarks.grid_row holds those since the last wva_grid_run / wva_grid_update
   bool force_lane_sizer = false;
   int gang_refill = -1;             // lock-step lane sizer: a warp refills only when all its lanes are idle; -1 = by size
   int length_sort = -1;             // lane sizer pulls items through the probe-sorted permutation (sizer_probe.cuh); -1 = by size
@@ -348,6 +381,8 @@ struct wva_ctx {
   int policy = 0;
   DevBuf sys_arena, cand_arena, sol_arena, scratch, gtab, greedy_ws, split_ws, order_ws, pool_ws;
   DevBuf marks, grid_marks, cycle_in, recalc_ws, gather_ws;   // wva_update_servers / wva_recalculate / wva_grid_update
+  DevBuf table_marks, pairs_ws;     // wva_update_tables: its marks (tmarks); the pair list of a table-marked update
+  TableMarks tmarks = {};
   PinBuf stage_in, stage_out;
   SysView sys = {};
   CandView cand = {};
@@ -465,27 +500,15 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   if (s->n_acc < 0 || s->n_types < 0 || s->n_models < 0 || s->n_servers < 0) return WVA_ERR_ARG;
   if (s->n_types > WVA_MAX_TYPES) { ctx->last_error = "wva_load_system: more than 64 capacity types"; return WVA_ERR_LIMIT; }
   CK(cudaSetDevice(ctx->device));
-  const size_t A = s->n_acc, T = s->n_types, M = s->n_models, S = s->n_servers, MA = M * A;
+  const size_t A = s->n_acc, T = s->n_types, M = s->n_models, S = s->n_servers;
   Ext n;
   n.A = A; n.T = T; n.M = M; n.S = S;
   Missing miss;
   each_sys(n, miss, ctx->sys, *s);
   if (miss.any) { ctx->last_error = "wva_load_system: a required array is NULL"; return WVA_ERR_ARG; }
   // validate indices the kernels dereference (after the NULL checks above)
-  for (size_t a = 0; a < A; a++)
-    if (s->acc_type[a] < 0 || s->acc_type[a] >= (int)T) { ctx->last_error = "wva_load_system: acc_type out of range"; return WVA_ERR_ARG; }
+  if (const char* bad = check_table_columns(*s, A, T, M)) { ctx->last_error = std::string("wva_load_system: ") + bad; return WVA_ERR_ARG; }
   if (const char* bad = check_server_columns(*s, S, (int)A, (int)M)) { ctx->last_error = std::string("wva_load_system: ") + bad; return WVA_ERR_ARG; }
-  // ServiceParms (pkg/analyzer/queueanalyzer.go:33-38) are measured service-time coefficients: finite and >= 0.  A
-  // negative or NaN coefficient makes arrival rates negative (QueueModel.Solve's gate, queuemodel.go:31) or NaN and
-  // the sizing meaningless; it is rejected here instead of being carried into the kernels.
-  for (size_t i = 0; i < MA; i++) {
-    if (!s->perf_present[i]) continue;
-    const float a = s->perf_alpha[i], b = s->perf_beta[i], g = s->perf_gamma[i];
-    if (!(a >= 0.0f && b >= 0.0f && g >= 0.0f) || a > 3.0e38f || b > 3.0e38f || g > 3.0e38f) {
-      ctx->last_error = "wva_load_system: perf_alpha / perf_beta / perf_gamma must be finite and >= 0";
-      return WVA_ERR_ARG;
-    }
-  }
   // one H2D copy of the whole arena, staged in pinned memory at the arena's offsets
   Layout L;
   each_sys(n, L, ctx->sys);
@@ -521,14 +544,15 @@ int32_t wva_load_system(wva_ctx* ctx, const wva_system* s) {
   ctx->loaded = true; ctx->calculated = false; ctx->solved = false;
   ctx->sized = false; ctx->marked = false;
   ctx->grid.current = false; ctx->grid_marked = false;
+  ctx->table_marked = false; ctx->table_grid_marked = false;
   return WVA_OK;
 }
 
 // ------------------------------------------------------------------ calculate
 }  // extern "C" (templates need C++ linkage)
 template <int THREADS, bool SMEM>
-static cudaError_t launch_sizer(wva_ctx* ctx, int mode, const SysView& sys_v, const CandView& cand_v, int blocks, size_t smem,
-                                unsigned long long n_pairs, int nmax, float* gtab, int* ovf_list) {
+static cudaError_t launch_sizer(wva_ctx* ctx, int mode, const SysView& sys_v, const CandView& cand_v, const int* list,
+                                int blocks, size_t smem, unsigned long long n_pairs, int nmax, float* gtab, int* ovf_list) {
   // mode 1 = flattened state machine (a burst of single chain states per round); 2 = lock-step rounds; 3 = lock-step
   // with two chains per lane; 4 = lock-step, every pair split into a TTFT item and an ITL item (mid-size systems); 5 =
   // split items whose second chain evaluates the predicted next bisection point (wva_core.cuh spec2_*)
@@ -565,8 +589,8 @@ static cudaError_t launch_sizer(wva_ctx* ctx, int mode, const SysView& sys_v, co
     });
     if (e != cudaSuccess) return e;
     const unsigned pb = (unsigned)((n_items + 127) / 128);
-    if (split) sizer_probe_kernel<true><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
-    else sizer_probe_kernel<false><<<pb, 128, 0, ctx->stream>>>(sys_v, n_items, nmax, k_in, v_in);
+    if (split) sizer_probe_kernel<true><<<pb, 128, 0, ctx->stream>>>(sys_v, list, n_items, nmax, k_in, v_in);
+    else sizer_probe_kernel<false><<<pb, 128, 0, ctx->stream>>>(sys_v, list, n_items, nmax, k_in, v_in);
     e = cub::DeviceRadixSort::SortPairsDescending(d_tmp, tmp, k_in, k_out, v_in, v_out, (int)n_items, 0, 32, ctx->stream);
     if (e != cudaSuccess) return e;
     ctx->launches += 4;
@@ -582,17 +606,18 @@ static cudaError_t launch_sizer(wva_ctx* ctx, int mode, const SysView& sys_v, co
                                    : sizer_lane_kernel<THREADS, SMEM, false, false, false>;
   e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  k<<<blocks, THREADS, smem, ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, gtab, ctx->d_ctr, ovf_list, sw, order, do_gang ? 1 : 0);
+  k<<<blocks, THREADS, smem, ctx->stream>>>(sys_v, cand_v, list, n_pairs, nmax, gtab, ctx->d_ctr, ovf_list, sw, order,
+                                            do_gang ? 1 : 0);
   ctx->launches++;
   return cudaGetLastError();
 }
 template <int WARPS>
-static cudaError_t launch_sizer_warp(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v, int blocks, size_t smem,
-                                     unsigned long long n_pairs, int nmax, int* ovf_list) {
+static cudaError_t launch_sizer_warp(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v, const int* list, int blocks,
+                                     size_t smem, unsigned long long n_pairs, int nmax, int* ovf_list) {
   auto k = sizer_warp_kernel<WARPS>;
   cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  k<<<blocks, WARPS * 32, smem, ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, ctx->d_ctr, ovf_list);
+  k<<<blocks, WARPS * 32, smem, ctx->stream>>>(sys_v, cand_v, list, n_pairs, nmax, ctx->d_ctr, ovf_list);
   ctx->launches++;
   return cudaGetLastError();
 }
@@ -629,11 +654,13 @@ int32_t wva_pool_phases(wva_ctx* ctx, uint64_t* out) {
 
 }  // extern "C"
 
-// CreateAllocation for every (server, accelerator) pair of the view sys_v into the rows of cand_v: the sizer picked by
-// the view's size, then the float64-overflow slow path.  Sets the sizer fields of ctx->timing (calculate_ms: ev[2] to
+// CreateAllocation for every (server, accelerator) pair of the view sys_v into the rows of cand_v, or, with a device
+// list of n_list pair indices of the view, for those pairs only (each written at its own row): the sizer picked by the
+// number of pairs, then the float64-overflow slow path.  Sets the sizer fields of ctx->timing (calculate_ms: ev[2] to
 // ev[3], the sizer launches).
-static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v) {
-  const unsigned long long n_pairs = (unsigned long long)sys_v.n_servers * ctx->A;
+static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& cand_v, const int* list = nullptr,
+                          unsigned long long n_list = 0) {
+  const unsigned long long n_pairs = list ? n_list : (unsigned long long)sys_v.n_servers * ctx->A;
   // scratch: counters + nmax reduction + overflow list.  The split sizer modes process a pair as TWO items and each may
   // append the pair (both chains of an alpha-dominated pair overflow at lambda_max): 2 entries per pair.
   int *d_nmax = nullptr, *d_ovf = nullptr;
@@ -645,7 +672,7 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
     // 1) largest batch size any pair will use -> table geometry
     int blocks = (int)((n_pairs + 255) / 256);
     if (blocks > 4096) blocks = 4096;
-    max_batch_kernel<<<blocks, 256, 0, ctx->stream>>>(sys_v, n_pairs, d_nmax);
+    max_batch_kernel<<<blocks, 256, 0, ctx->stream>>>(sys_v, list, n_pairs, d_nmax);
     ctx->launches++;
     int nmax = 0;
     CK(cudaMemcpyAsync(&nmax, d_nmax, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -673,8 +700,8 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
       CK(ctx->pool_ws.reserve(pool_bytes + 512));
       PoolEntry* pool = (PoolEntry*)ctx->pool_ws.p;
       CK(cudaFuncSetAttribute(sizer_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PoolSmem)));
-      sizer_pool_kernel<<<ctx->sm_count, POOL_THREADS, sizeof(PoolSmem), ctx->stream>>>(sys_v, cand_v, n_pairs, nmax, P, pool,
-                                                                                        ctx->d_ctr, d_ovf);
+      sizer_pool_kernel<<<ctx->sm_count, POOL_THREADS, sizeof(PoolSmem), ctx->stream>>>(sys_v, cand_v, list, n_pairs, nmax, P,
+                                                                                        pool, ctx->d_ctr, d_ovf);
       ctx->launches++;
       cudaError_t pe = cudaGetLastError();
       if (pe != cudaSuccess) { ctx->last_error = std::string("pool sizer launch: ") + cudaGetErrorString(pe); return WVA_ERR_CUDA; }
@@ -686,10 +713,10 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
       ctx->timing.sizer_kernel = 1;
       if (warp_tab * 8 <= 48 * 1024) {
         int per_sm = (int)(SMEM_PER_SM / (warp_tab * 8 + 1024)); if (per_sm > 6) per_sm = 6; if (per_sm < 1) per_sm = 1;
-        e = launch_sizer_warp<8>(ctx, sys_v, cand_v, ctx->sm_count * per_sm, warp_tab * 8, n_pairs, nmax, d_ovf);
+        e = launch_sizer_warp<8>(ctx, sys_v, cand_v, list, ctx->sm_count * per_sm, warp_tab * 8, n_pairs, nmax, d_ovf);
       } else {
         int per_sm = (int)(SMEM_PER_SM / (warp_tab * 4 + 1024)); if (per_sm > 8) per_sm = 8; if (per_sm < 1) per_sm = 1;
-        e = launch_sizer_warp<4>(ctx, sys_v, cand_v, ctx->sm_count * per_sm, warp_tab * 4, n_pairs, nmax, d_ovf);
+        e = launch_sizer_warp<4>(ctx, sys_v, cand_v, list, ctx->sm_count * per_sm, warp_tab * 4, n_pairs, nmax, d_ovf);
       }
     } else {
       // The lane sizer.  Its head table (4 B x nmax per lane) lives in shared memory when at least 64 lanes fit on an
@@ -721,16 +748,16 @@ static int32_t size_views(wva_ctx* ctx, const SysView& sys_v, const CandView& ca
         size_t smem = per_lane * best_threads;
         ctx->timing.sizer_kernel = 2;
         switch (best_threads) {
-          case 256: e = launch_sizer<256, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-          case 192: e = launch_sizer<192, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-          case 128: e = launch_sizer<128, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
-          default: e = launch_sizer<64, true>(ctx, mode, sys_v, cand_v, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          case 256: e = launch_sizer<256, true>(ctx, mode, sys_v, cand_v, list, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          case 192: e = launch_sizer<192, true>(ctx, mode, sys_v, cand_v, list, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          case 128: e = launch_sizer<128, true>(ctx, mode, sys_v, cand_v, list, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
+          default: e = launch_sizer<64, true>(ctx, mode, sys_v, cand_v, list, blocks, smem, n_pairs, nmax, nullptr, d_ovf); break;
         }
       } else {
         int blk = ctx->sm_count * 2;
         ctx->timing.sizer_kernel = 3;
         CK(ctx->gtab.reserve((size_t)blk * 256 * per_lane));
-        e = launch_sizer<256, false>(ctx, mode, sys_v, cand_v, blk, 0, n_pairs, nmax, (float*)ctx->gtab.p, d_ovf);
+        e = launch_sizer<256, false>(ctx, mode, sys_v, cand_v, list, blk, 0, n_pairs, nmax, (float*)ctx->gtab.p, d_ovf);
       }
     }
     if (e != cudaSuccess) { ctx->last_error = std::string("sizer launch: ") + cudaGetErrorString(e); return WVA_ERR_CUDA; }
@@ -772,6 +799,7 @@ int32_t wva_calculate(wva_ctx* ctx) {
   if (rc != WVA_OK) return rc;
   ctx->calculated = true; ctx->solved = false;
   ctx->sized = true; ctx->marked = false;   // every pair sized from the resident columns: the marks are void
+  ctx->table_marked = false;
   ctx->shard_status = WVA_OK;
   return WVA_OK;
 }
@@ -841,6 +869,27 @@ static void launch_move_rows(wva_ctx* ctx, const RowMoves& m, const int* rows, i
   ctx->launches++;
 }
 
+// The pairs of the rank's block that `pred` selects, compacted in pair order into ctx->pairs_ws as indices into the
+// block: *list and *n_list.
+static int32_t select_pairs(wva_ctx* ctx, const TablePair& pred, int** list, int* n_list) {
+  *n_list = 0;
+  const long long n_pairs = (long long)(ctx->shard_hi - ctx->shard_lo) * ctx->A;
+  if (n_pairs == 0) return WVA_OK;
+  if (n_pairs > 0x7fffffffLL) { ctx->last_error = "a block of more than 2^31 - 1 pairs takes no pair list"; return WVA_ERR_LIMIT; }
+  thrust::counting_iterator<int> pairs(0);
+  size_t tmp = 0;
+  CK(cub::DeviceSelect::If(nullptr, tmp, pairs, (int*)nullptr, (int*)nullptr, (int)n_pairs, pred, ctx->stream));
+  int* d_cnt = nullptr;
+  unsigned char* d_tmp = nullptr;
+  Layout L;
+  CK(lay_out(ctx->pairs_ws, L, [&](Layout& f) { f(n_pairs, 0, *list); f(1, 0, d_cnt); f(tmp, 0, d_tmp); }));
+  CK(cub::DeviceSelect::If(d_tmp, tmp, pairs, *list, d_cnt, (int)n_pairs, pred, ctx->stream));
+  ctx->launches++;
+  CK(cudaMemcpyAsync(n_list, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return WVA_OK;
+}
+
 extern "C" {
 
 int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
@@ -862,8 +911,8 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
   // 1) the rank's marked servers compacted, in server order: the re-size list, then the re-value-only list
   int cnt[2] = {0, 0};
   int *resize = nullptr, *revalue = nullptr;
-  if (ctx->marked && n > 0) {
-    const unsigned char* marks = (const unsigned char*)ctx->marks.p;
+  const unsigned char* marks = ctx->marked && n > 0 ? (const unsigned char*)ctx->marks.p : nullptr;
+  if (marks) {
     thrust::counting_iterator<int> servers(lo);
     thrust::discard_iterator<> clean;
     size_t tmp = 0;
@@ -876,13 +925,31 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
     CK(cub::DevicePartition::If(d_tmp, tmp, servers, resize, revalue, clean, d_cnt, n, MarkedResize{marks},
                                 MarkedRevalueOnly{marks}, ctx->stream));
     ctx->launches++;
-    CK(cudaMemsetAsync(ctx->marks.p, 0, ctx->S, ctx->stream));
     CK(cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
-  ctx->marked = false;
   const int D = cnt[0], R = cnt[1];
-  if (D > 0) {
+  // the current allocation alone changed: TransitionPenalty of every candidate again (before any re-sizing, which writes
+  // its pairs' values itself)
+  auto revalue_servers = [&]() {
+    if (R == 0 || A == 0) return;
+    const unsigned long long n_items = (unsigned long long)R * A;
+    const unsigned long long blocks = std::min<unsigned long long>((n_items + 255) / 256, (unsigned long long)ctx->sm_count * 16);
+    revalue_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(ctx->sys, ctx->cand, revalue, n_items);
+    ctx->launches++;
+  };
+  if (ctx->table_marked) {
+    // 2) table marks: every pair of a re-size-marked server and the table-marked pairs of the others, sized in place
+    revalue_servers();
+    const SysView blk = shard_sys(ctx);
+    const TablePair pred{blk.srv_model, marks ? marks + lo : nullptr, MARK_RESIZE, ctx->tmarks.size_row,
+                         ctx->tmarks.size_acc, A};
+    int* list = nullptr;
+    int n_list = 0;
+    int32_t rc = select_pairs(ctx, pred, &list, &n_list);
+    if (rc == WVA_OK && n_list > 0) rc = size_views(ctx, blk, shard_cand(ctx), list, (unsigned long long)n_list);
+    if (rc != WVA_OK) return rc;
+  } else if (D > 0) {
     // 2) the D servers' columns gathered into a view of D servers (model, perf and accelerator arrays shared) ...
     Ext g;
     g.S = (size_t)D; g.P = (size_t)D * A;
@@ -905,13 +972,9 @@ int32_t wva_recalculate(wva_ctx* ctx, int64_t* n_resized, int64_t* n_revalued) {
     each_cand(g, AddMove{out}, gcand, ctx->cand);
     launch_move_rows(ctx, out, resize, D, A, true);
   }
-  // 5) the current allocation alone changed: TransitionPenalty of every candidate again
-  if (R > 0 && A > 0) {
-    const unsigned long long n_items = (unsigned long long)R * A;
-    const unsigned long long blocks = std::min<unsigned long long>((n_items + 255) / 256, (unsigned long long)ctx->sm_count * 16);
-    revalue_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(ctx->sys, ctx->cand, revalue, n_items);
-    ctx->launches++;
-  }
+  if (!ctx->table_marked) revalue_servers();
+  if (marks) CK(cudaMemsetAsync(ctx->marks.p, 0, ctx->S, ctx->stream));
+  ctx->marked = false; ctx->table_marked = false;
   CK(cudaGetLastError());
   CK(cudaEventRecord(ctx->ev[3], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
@@ -1077,6 +1140,66 @@ int32_t wva_update_server_set(wva_ctx* ctx, int32_t n_servers, const int32_t* pr
   CK(cudaStreamSynchronize(ctx->stream));   // the staging buffer is free for the next call
   ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
   ctx->marked = true; ctx->grid_marked = true; ctx->solved = false;
+  return WVA_OK;
+}
+
+// ------------------------------------------------------------------ table update
+int32_t wva_update_tables(wva_ctx* ctx, const wva_system* tables, int64_t* n_marked) {
+  if (!ctx) return WVA_ERR_ARG;
+  if (n_marked) *n_marked = 0;
+  if (!ctx->loaded) { ctx->last_error = "wva_update_tables before wva_load_system"; return WVA_ERR_STATE; }
+  auto bad_arg = [&](const char* why) { ctx->last_error = std::string("wva_update_tables: ") + why; return WVA_ERR_ARG; };
+  if (!tables) return bad_arg("tables is NULL");
+  if (tables->n_acc != ctx->A || tables->n_types != ctx->T || tables->n_models != ctx->M)
+    return bad_arg("n_acc, n_types and n_models must be the loaded system's");
+  const size_t A = (size_t)ctx->A, M = (size_t)ctx->M, MA = M * A;
+  if (const char* bad = check_table_columns(*tables, A, (size_t)ctx->T, M)) return bad_arg(bad);
+  CK(cudaSetDevice(ctx->device));
+  // the table columns staged at their offsets of one pinned buffer, one H2D copy, then one classify-and-write pass
+  SysView nu = ctx->sys;
+  Layout L;
+  each_table(A, M, L, nu);
+  const size_t total = L.off + 256;
+  CK(ctx->stage_in.reserve(total));
+  CK(ctx->cycle_in.reserve(total));
+  TableMarks& tm = ctx->tmarks;
+  Layout TL;
+  CK(lay_out(ctx->table_marks, TL, [&](Layout& f) { f(MA, 0, tm.size_row); f(A, 0, tm.size_acc); f(MA, 0, tm.grid_row); f(MA + A, 0, tm.fresh); }));
+  unsigned long long* d_count = nullptr;
+  Layout W;
+  CK(lay_out(ctx->pairs_ws, W, [&](Layout& f) { f(1, 0, d_count); }));
+  char* h = (char*)ctx->stage_in.p;
+  L = Layout{(char*)ctx->cycle_in.p};
+  each_table(A, M, [&](size_t c, int, auto*& d, auto* src) { if (c) memcpy(h + L.off, src, c * sizeof(*d)); L(c, 0, d); }, nu, *tables);
+  CK(cudaEventRecord(ctx->ev[0], ctx->stream));
+  CK(cudaMemcpyAsync(ctx->cycle_in.p, h, total, cudaMemcpyHostToDevice, ctx->stream));
+  if (!ctx->table_marked) {
+    CK(cudaMemsetAsync(tm.size_row, 0, MA, ctx->stream));
+    CK(cudaMemsetAsync(tm.size_acc, 0, A, ctx->stream));
+  }
+  if (!ctx->table_grid_marked) CK(cudaMemsetAsync(tm.grid_row, 0, MA, ctx->stream));
+  CK(cudaMemsetAsync(d_count, 0, sizeof(*d_count), ctx->stream));
+  const size_t items = std::max(MA, A);
+  if (items > 0) {
+    classify_tables_kernel<<<(unsigned)((items + 255) / 256), 256, 0, ctx->stream>>>(ctx->sys, nu, (int)A, (int)M, tm);
+    ctx->launches++;
+  }
+  // the pairs of the block this diff marked for re-sizing
+  const SysView blk = shard_sys(ctx);
+  const unsigned long long n_pairs = (unsigned long long)blk.n_servers * A;
+  if (n_pairs > 0) {
+    count_table_pairs_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, ctx->stream>>>(blk.srv_model, (int)A, (int)M, n_pairs,
+                                                                                       tm.fresh, d_count);
+    ctx->launches++;
+  }
+  unsigned long long count = 0;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(ctx->ev[1], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));   // the staging buffer is free for the next call
+  ctx->timing.h2d_ms = elapsed(ctx, 0, 1);
+  ctx->table_marked = true; ctx->table_grid_marked = true; ctx->solved = false;
+  if (n_marked) *n_marked = (int64_t)count;
   return WVA_OK;
 }
 

@@ -72,9 +72,9 @@ struct GridSide {            // what an evaluation needs of its pair
   float total_rate, slo_ttft, slo_itl, slo_tps, lambda_tps;
   int pad_[3];
 };
-struct GridDefer {
+struct GridDefer {            // indexed by the launch's work items: its pairs, or positions in its pair list
   GridSide* side;            // [n_pairs], nullptr = no deferral
-  unsigned long long* items; // (pair << 16) | r
+  unsigned long long* items; // (item << 16) | r
   unsigned char* cls;        // length class of the item (sort key)
   unsigned long long* n_items;
   unsigned long long cap;
@@ -144,10 +144,12 @@ __device__ unsigned long long g_grid_phase[GPH_N];
 #define GRID_PH(...)
 #endif
 
-template <int WARPS>
+// LISTED: the work items are entries of `list` (list_pair); a launch without a list runs the instance that never reads
+// it, which keeps the pointer out of the <8> instance's 128-register budget
+template <int WARPS, bool LISTED>
 __global__ void __launch_bounds__(WARPS * 32, WARPS == 8 ? 2 : 1)
-grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax, GridCounters* ctr, GridDefer df,
-            GridOverflowList ol) {
+grid_kernel(SysView s, int R, GridOut out, const int* list, unsigned long long n_pairs, int nmax, GridCounters* ctr,
+            GridDefer df, GridOverflowList ol) {
   extern __shared__ double2 smem_grid[];
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -158,10 +160,11 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
 
   while (true) {
     GRID_PH(const long long ph_t0 = clock64();)
-    unsigned long long pair = 0;
-    if (lane == 0) pair = atomicAdd(&ctr->next_pair, 1ull);
-    pair = __shfl_sync(full, pair, 0);
-    if (pair >= n_pairs) break;
+    unsigned long long item = 0;
+    if (lane == 0) item = atomicAdd(&ctr->next_pair, 1ull);
+    item = __shfl_sync(full, item, 0);
+    if (item >= n_pairs) break;
+    const unsigned long long pair = list_pair(LISTED ? list : nullptr, item);
     const int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
     const size_t obase = (size_t)pair * (size_t)R;
     PairModel m;
@@ -192,7 +195,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
     grid_model_finish(m, tabf);
     const float lambda_tps = f_mul(m.lambda_max, f_sub(1.0f, WVA_STABILITY_SAFETY));
     int front = 0x7fffffff;
-    const bool deferring = df.side != nullptr && pair < 0xffffffffull;
+    const bool deferring = df.side != nullptr && item < 0xffffffffull;
     bool saved = false;                                   // the pair's model is written when its first level is deferred
     const float mu_last_f = (float)m.mu_last;
     bool first_round = true;
@@ -243,7 +246,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
             defer[c] = want && rank < room;
             if (defer[c]) {
               const unsigned long long k = base + rank;
-              df.items[k] = (pair << 16) | (unsigned long long)r[c];
+              df.items[k] = (item << 16) | (unsigned long long)r[c];
               df.cls[k] = (unsigned char)grid_class(m, ratio);
             }
             if (room > 0 && !saved) {                       // warp-uniform: the first level of the pair that leaves
@@ -252,7 +255,7 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
                 GridSide sd;
                 sd.m = m; sd.m.tab = nullptr; sd.m.stride = 0;
                 sd.total_rate = total_rate; sd.slo_ttft = slo_ttft; sd.slo_itl = slo_itl; sd.slo_tps = slo_tps; sd.lambda_tps = lambda_tps;
-                df.side[pair] = sd;
+                df.side[item] = sd;
               }
             }
           }
@@ -333,8 +336,8 @@ grid_kernel(SysView s, int R, GridOut out, unsigned long long n_pairs, int nmax,
 
 // The deferred levels, sorted by length class: lane per (pair, level), 32 different pairs per warp.
 __global__ void __launch_bounds__(256, 2)
-grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long* __restrict__ items, unsigned long long n_items,
-                     GridCounters* ctr, unsigned long long* next_item, GridOverflowList ol) {
+grid_deferred_kernel(int R, GridOut out, const int* list, GridDefer df, const unsigned long long* __restrict__ items,
+                     unsigned long long n_items, GridCounters* ctr, unsigned long long* next_item, GridOverflowList ol) {
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   unsigned long long my_solves = 0, my_states = 0, my_slots = 0, my_rounds = 0;
@@ -345,9 +348,9 @@ grid_deferred_kernel(int R, GridOut out, GridDefer df, const unsigned long long*
     if (i0 >= n_items) break;
     const bool live = i0 + lane < n_items;
     unsigned long long it = live ? items[i0 + lane] : items[i0];
-    const unsigned long long pair = it >> 16;
+    const unsigned long long pair = list_pair(list, it >> 16);
     const int r = (int)(it & 0xffffu);
-    const GridSide* sp = df.side + pair;
+    const GridSide* sp = df.side + (it >> 16);
     PairModel m = sp->m;
     const float total_rate = sp->total_rate, slo_ttft = sp->slo_ttft, slo_itl = sp->slo_itl, slo_tps = sp->slo_tps,
                 lambda_tps = sp->lambda_tps;
@@ -427,9 +430,11 @@ __global__ void __launch_bounds__(64) grid_overflow_kernel(SysView s, int R, Gri
   if (grid_store(out, o, m, st, lambda, slo_ttft, slo_itl, slo_tps, lambda_tps) && out.frontier) atomicMin(&out.frontier[pair], r);
 }
 
-__global__ void __launch_bounds__(256) grid_frontier_fix_kernel(int* frontier, unsigned long long n) {
-  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && frontier[i] == 0x7fffffff) frontier[i] = 0;
+__global__ void __launch_bounds__(256) grid_frontier_fix_kernel(int* frontier, const int* list, unsigned long long n) {
+  const unsigned long long item = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (item >= n) return;
+  const unsigned long long i = list_pair(list, item);
+  if (frontier[i] == 0x7fffffff) frontier[i] = 0;
 }
 
 }  // namespace wva

@@ -64,7 +64,7 @@ static inline int32_t run_overflow_slow_path(const SysView& s, const CandView& o
   if (cudaMalloc(&d_nmax, 8) != cudaSuccess) return 1;
   cudaMemsetAsync(d_nmax, 0, 8, stream);
   unsigned long long n_pairs = (unsigned long long)s.n_servers * s.n_acc;
-  max_batch_kernel<<<1024, 256, 0, stream>>>(s, n_pairs, d_nmax);
+  max_batch_kernel<<<1024, 256, 0, stream>>>(s, nullptr, n_pairs, d_nmax);
   (*launches)++;
   cudaMemcpyAsync(&nmax_h, d_nmax, 4, cudaMemcpyDeviceToHost, stream);
   cudaStreamSynchronize(stream);

@@ -80,6 +80,79 @@ struct MarkedRevalueOnly {
   __device__ bool operator()(int i) const { return marks[i] == MARK_REVALUE; }
 };
 
+// The marks of wva_update_tables, keyed by table row so that a change of the server set leaves them valid.  size_row /
+// size_acc accumulate until the next wva_calculate / wva_recalculate, grid_row until the next wva_grid_run /
+// wva_grid_update; fresh holds the last call's own sizing diff ([M*A] rows, then [A] costs) for its count.
+struct TableMarks {
+  unsigned char *size_row, *size_acc, *grid_row, *fresh;
+};
+
+// One pass over the table entries of `nu` (thread t: perf row t of [M*A] and accelerator t of [A]): the bitwise diff
+// against the resident tables `res`, the write of `nu` over them, and the marks.  A perf row is marked for sizing when
+// a field sizer_setup / alloc_final reads changed (alpha, beta, gamma, max_batch, at_tokens, acc_count, present) and
+// for the grid when one grid_setup reads changed (all of them but acc_count); an accelerator for sizing when its cost
+// changed (every candidate's cost and value).  acc_multiplicity and acc_type are written and mark nothing: only the
+// allocators read them.
+__global__ void classify_tables_kernel(SysView res, SysView nu, int A, int M, TableMarks tm) {
+  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  const long long MA = (long long)M * A;
+  if (t < MA) {
+    const float al = nu.perf_alpha[t], be = nu.perf_beta[t], ga = nu.perf_gamma[t];
+    const int mb = nu.perf_max_batch[t], at = nu.perf_at_tokens[t], ac = nu.perf_acc_count[t];
+    const unsigned char pr = nu.perf_present[t];
+    const bool grid = bits_differ(al, res.perf_alpha[t]) || bits_differ(be, res.perf_beta[t]) ||
+                      bits_differ(ga, res.perf_gamma[t]) || mb != res.perf_max_batch[t] || at != res.perf_at_tokens[t] ||
+                      pr != res.perf_present[t];
+    const bool size = grid || ac != res.perf_acc_count[t];
+    const_cast<float*>(res.perf_alpha)[t] = al;
+    const_cast<float*>(res.perf_beta)[t] = be;
+    const_cast<float*>(res.perf_gamma)[t] = ga;
+    const_cast<int*>(res.perf_max_batch)[t] = mb;
+    const_cast<int*>(res.perf_at_tokens)[t] = at;
+    const_cast<int*>(res.perf_acc_count)[t] = ac;
+    const_cast<unsigned char*>(res.perf_present)[t] = pr;
+    if (size) tm.size_row[t] = 1;
+    if (grid) tm.grid_row[t] = 1;
+    tm.fresh[t] = size;
+  }
+  if (t < A) {
+    const float cost = nu.acc_cost[t];
+    const bool changed = bits_differ(cost, res.acc_cost[t]);
+    const_cast<float*>(res.acc_cost)[t] = cost;
+    const_cast<int*>(res.acc_multiplicity)[t] = nu.acc_multiplicity[t];
+    const_cast<int*>(res.acc_type)[t] = nu.acc_type[t];
+    if (changed) tm.size_acc[t] = 1;
+    tm.fresh[MA + t] = changed;
+  }
+}
+
+// Pair t of a block view (server t / A, accelerator t % A) is listed when its server carries `bit` in srv_marks (the
+// block's server marks, NULL = none pending), or when the server's model is known and its perf row (model, acc) is in
+// `row` or its accelerator in `acc` (NULL = no accelerator marks).  Unknown-model servers read no table.
+struct TablePair {
+  const int* srv_model;
+  const unsigned char* srv_marks;
+  unsigned char bit;
+  const unsigned char *row, *acc;
+  int A;
+  __device__ bool operator()(int t) const {
+    const int srv = t / A, a = t % A;
+    if (srv_marks && (srv_marks[srv] & bit)) return true;
+    const int m = srv_model[srv];
+    return m >= 0 && (row[(size_t)m * A + a] || (acc && acc[a]));
+  }
+};
+
+// The pairs of the block view's n_pairs whose perf row or accelerator the last wva_update_tables changed (fresh), summed
+// into *count.
+__global__ void __launch_bounds__(256) count_table_pairs_kernel(const int* srv_model, int A, int M, unsigned long long n_pairs,
+                                                                const unsigned char* fresh, unsigned long long* count) {
+  const unsigned long long t = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  const TablePair marked{srv_model, nullptr, 0, fresh, fresh + (size_t)M * A, A};
+  const unsigned hit = __ballot_sync(0xffffffffu, t < n_pairs && marked((int)t));
+  if ((threadIdx.x & 31) == 0 && hit) atomicAdd(count, (unsigned long long)__popc(hit));
+}
+
 // Per-server rows of up to 32 columns moved between a resident arena and a compacted one: row rows[i] of the resident
 // columns <-> row i of the compacted ones, `per` elements per row (1 for server columns, A for candidate rows).
 struct RowMoves {

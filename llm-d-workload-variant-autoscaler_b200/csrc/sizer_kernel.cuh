@@ -29,11 +29,12 @@ __device__ __forceinline__ void retire_overflow(SizerLane& z, const SysView& s, 
 }
 
 // Largest max-batch-size N any pair that needs sizing will use (allocation.go:79-88):
-// decides the table geometry of the sizer launch.
-__global__ void __launch_bounds__(256) max_batch_kernel(SysView s, unsigned long long n_pairs, int* out) {
+// decides the table geometry of the sizer launch.  Items are pairs of the view, or entries of `list` (list_pair).
+__global__ void __launch_bounds__(256) max_batch_kernel(SysView s, const int* list, unsigned long long n_pairs, int* out) {
   int best = 0;
-  for (unsigned long long pair = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; pair < n_pairs;
-       pair += (unsigned long long)gridDim.x * blockDim.x) {
+  for (unsigned long long item = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; item < n_pairs;
+       item += (unsigned long long)gridDim.x * blockDim.x) {
+    const unsigned long long pair = list_pair(list, item);
     int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
     int model = s.srv_model[srv];
     if (model < 0) continue;

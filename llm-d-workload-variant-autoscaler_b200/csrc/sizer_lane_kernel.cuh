@@ -16,22 +16,23 @@
 
 namespace wva {
 
-// Split mode scratch: per pair two published results + a completion counter (zeroed before the launch).
+// Split mode scratch: per work pair (the pair, or its position in the launch's list) two published results + a
+// completion counter (zeroed before the launch).
 struct SplitWs {
   float* res;     // [2 * n_pairs] lambda* of the TTFT / ITL item, < 0 = the search failed
   int* solves;    // [2 * n_pairs]
   int* cnt;       // [n_pairs]
 };
 
-// A split item finished its search: publish; the first finisher retires, the second merges and goes on.
+// A split item (`me` = 2 * work pair + kind) finished its search: publish; the first finisher retires, the second
+// merges and goes on.
 template <bool DUAL>
-__device__ __forceinline__ bool split_publish(SizerLane& z, const SysView& s, const CandView& out, const SplitWs& sw) {
-  const size_t pair = (size_t)z.srv * s.n_acc + z.acc;
-  const size_t me = pair * 2 + (size_t)z.split;
+__device__ __forceinline__ bool split_publish(SizerLane& z, const SysView& s, const CandView& out, const SplitWs& sw,
+                                              unsigned long long me) {
   sw.res[me] = z.failed ? -1.0f : (z.split == 0 ? z.sT.result : z.sI.result);
   sw.solves[me] = z.solves;
   __threadfence();
-  const int old = atomicAdd(&sw.cnt[pair], 1);
+  const int old = atomicAdd(&sw.cnt[me >> 1], 1);
   if (old == 0) return false;                          // partner still searching: it will finish the pair
   __threadfence();
   const float pr = *((volatile float*)&sw.res[me ^ 1]);
@@ -48,7 +49,7 @@ __device__ __forceinline__ bool split_publish(SizerLane& z, const SysView& s, co
 // its rounds are not counted in lockstep_slots.
 template <int THREADS, bool SMEM_TABLE, bool DUAL, bool SPLIT, bool FLAT>
 __device__ __forceinline__ void
-sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
+sizer_lane_body(SysView s, CandView out, const int* list, unsigned long long n_pairs, int nmax, float* gtab,
                   SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {
   static_assert(!FLAT || (!DUAL && !SPLIT), "the flattened round runs whole pairs, one chain per lane");
   extern __shared__ float smem_tab[];
@@ -63,6 +64,7 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
   z.m.N = 1; z.m.K = 11; z.m.mono = 0; z.m.mu_last = 1.0; z.m.r_last = 1.0;
   SolveStats st;
   bool live = false, exhausted = false;
+  unsigned long long my_item = 0;   // the lane's item (SPLIT: its split_publish slot)
   unsigned long long my_solves = 0, my_states = 0, my_slots = 0;
 
   while (true) {
@@ -77,12 +79,12 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
         unsigned long long item = atomicAdd(&ctr->next_pair, 1ull);
         if (item >= (SPLIT ? 2 * n_pairs : n_pairs)) { exhausted = true; break; }
         if (order) item = order[item];                 // length-sorted queue (sizer_probe.cuh)
-        const unsigned long long pair = SPLIT ? (item >> 1) : item;
+        const unsigned long long pair = list_pair(list, SPLIT ? (item >> 1) : item);
         int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
         int lim = 0;
         int rc = sizer_setup(z, s, out, srv, acc, nmax, &lim, !SPLIT || (item & 1) == 0);
         if (lim) ctr->limit_hit = 1;
-        if (rc == SETUP_NEEDS_TABLE) { need_table = true; if (SPLIT) z.split = (int)(item & 1); break; }
+        if (rc == SETUP_NEEDS_TABLE) { need_table = true; if (SPLIT) { z.split = (int)(item & 1); my_item = item; } break; }
       }
     }
     // ---- BuildModel, cooperatively: the warp fills each requesting lane's column ----------------
@@ -97,7 +99,7 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
     if (need_table) {
       model_finish(z.m, tab, stride);
       live = DUAL ? (SPLIT ? spec2_begin(z, s, out) : dual_begin(z, s, out)) : sizer_begin(z, s, out);
-      if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<DUAL>(z, s, out, sw); }
+      if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<DUAL>(z, s, out, sw, my_item); }
       if (!live) my_solves += z.solves;
     }
     const unsigned live_mask = __ballot_sync(full, live);
@@ -161,7 +163,7 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
         live = false;
       } else {
         live = DUAL ? (SPLIT ? spec2_on_solve(z, s, out, st2, sv) : dual_on_solve(z, s, out, st2, sv)) : sizer_on_solve(z, s, out, st);
-        if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<DUAL>(z, s, out, sw); }
+        if (SPLIT) { if (live && z.stage == SZ_PUBLISH) live = split_publish<DUAL>(z, s, out, sw, my_item); }
       }
       if (!live) { my_solves += z.solves; my_states += z.states; }
     }
@@ -183,9 +185,10 @@ sizer_lane_body(SysView s, CandView out, unsigned long long n_pairs, int nmax, f
 
 template <int THREADS, bool SMEM_TABLE, bool DUAL, bool SPLIT, bool FLAT>
 __global__ void __launch_bounds__(THREADS)
-sizer_lane_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
+sizer_lane_kernel(SysView s, CandView out, const int* list, unsigned long long n_pairs, int nmax, float* gtab,
                   SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {
-  sizer_lane_body<THREADS, SMEM_TABLE, DUAL, SPLIT, FLAT>(s, out, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
+  sizer_lane_body<THREADS, SMEM_TABLE, DUAL, SPLIT, FLAT>(s, out, list, n_pairs, nmax, gtab, ctr, overflow_list, sw, order,
+                                                          gang);
 }
 
 // The plain lane kernel with its table in global memory — large N on large systems (BASELINE config 3) — is launched
@@ -193,9 +196,9 @@ sizer_lane_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
 // 128 registers (spills only around the solver call, none in the chunk loops) both blocks run: 4 warps per SMSP feed
 // the FP64 pipe instead of 2.
 __global__ void __launch_bounds__(256, 2)
-sizer_lane_kernel_gtab_2blk(SysView s, CandView out, unsigned long long n_pairs, int nmax, float* gtab,
+sizer_lane_kernel_gtab_2blk(SysView s, CandView out, const int* list, unsigned long long n_pairs, int nmax, float* gtab,
                             SizerCounters* ctr, int* overflow_list, SplitWs sw, const unsigned* order, int gang) {
-  sizer_lane_body<256, false, false, false, false>(s, out, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
+  sizer_lane_body<256, false, false, false, false>(s, out, list, n_pairs, nmax, gtab, ctr, overflow_list, sw, order, gang);
 }
 
 }  // namespace wva

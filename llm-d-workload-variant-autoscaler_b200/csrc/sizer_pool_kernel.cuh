@@ -154,7 +154,7 @@ __device__ __noinline__ bool pool_pair_on_chain(PoolEntry& ze, const SysView& s,
 }
 
 __global__ void __launch_bounds__(POOL_THREADS, 1)
-sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, int P, PoolEntry* pool_all,
+sizer_pool_kernel(SysView s, CandView out, const int* list, unsigned long long n_pairs, int nmax, int P, PoolEntry* pool_all,
                   SizerCounters* ctr, int* overflow_list) {
   extern __shared__ __align__(16) unsigned char pool_smem_raw[];
   PoolSmem& sm = *reinterpret_cast<PoolSmem*>(pool_smem_raw);
@@ -270,8 +270,9 @@ sizer_pool_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
       bool need_table = false;
       if (new_slot >= 0) {
         while (true) {
-          const unsigned long long pair = atomicAdd(&ctr->next_pair, 1ull);
-          if (pair >= n_pairs) { sm.exhausted = 1; break; }
+          const unsigned long long item = atomicAdd(&ctr->next_pair, 1ull);
+          if (item >= n_pairs) { sm.exhausted = 1; break; }
+          const unsigned long long pair = list_pair(list, item);
           const int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
           int lim = 0;
           const int rc = sizer_setup(z, s, out, srv, acc, nmax, &lim, true);

@@ -112,12 +112,15 @@ WVA_HD unsigned probe_item_key(const SysView& s, unsigned long long item, bool s
 }
 
 #if defined(__CUDACC__)
+// keys[item] for every item of the launch; with a pair list the items are list positions (ids stay positions, which is
+// what the lane sizer's queue holds) and each is probed as the item of its listed pair
 template <bool SPLIT>
-__global__ void __launch_bounds__(128) sizer_probe_kernel(SysView s, unsigned long long n_items, int nmax, unsigned* keys,
-                                                          unsigned* ids) {
+__global__ void __launch_bounds__(128) sizer_probe_kernel(SysView s, const int* list, unsigned long long n_items, int nmax,
+                                                          unsigned* keys, unsigned* ids) {
   const unsigned long long item = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= n_items) return;
-  keys[item] = probe_item_key(s, item, SPLIT, nmax);
+  const unsigned long long probed = SPLIT ? 2 * list_pair(list, item >> 1) + (item & 1) : list_pair(list, item);
+  keys[item] = probe_item_key(s, probed, SPLIT, nmax);
   ids[item] = (unsigned)item;
 }
 

@@ -45,7 +45,8 @@ __device__ __forceinline__ void warp_solve(const PairModel& m, const double2* ta
 
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
-sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax, SizerCounters* ctr, int* overflow_list) {
+sizer_warp_kernel(SysView s, CandView out, const int* list, unsigned long long n_pairs, int nmax, SizerCounters* ctr,
+                  int* overflow_list) {
   extern __shared__ double2 smem_tab2[];
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -56,10 +57,11 @@ sizer_warp_kernel(SysView s, CandView out, unsigned long long n_pairs, int nmax,
   unsigned long long my_solves = 0;
 
   while (true) {
-    unsigned long long pair = 0;
-    if (lane == 0) pair = atomicAdd(&ctr->next_pair, 1ull);
-    pair = __shfl_sync(full, pair, 0);
-    if (pair >= n_pairs) break;
+    unsigned long long item = 0;
+    if (lane == 0) item = atomicAdd(&ctr->next_pair, 1ull);
+    item = __shfl_sync(full, item, 0);
+    if (item >= n_pairs) break;
+    const unsigned long long pair = list_pair(list, item);
     const int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
     SizerLane z;   // used for its setup / bookkeeping fields; every lane holds the same copy
     int lim = 0;

@@ -656,6 +656,13 @@ struct CandView {  // device image of wva_candidates, row-major [S][A]
   int* n_solves;
 };
 
+// The pair of a view a kernel's work item `item` stands for: the item itself, or, when the launch is handed a list of
+// pairs (wva_recalculate / wva_grid_update after wva_update_tables), the list's entry.  Results are written at the
+// pair's own row, so a listed launch updates those rows in place.
+WVA_HD unsigned long long list_pair(const int* list, unsigned long long item) {
+  return list ? (unsigned long long)list[item] : item;
+}
+
 struct Alloc {  // core.Allocation (pkg/core/allocation.go:13-24)
   int state; long long num_replicas; int batch_size;
   float cost, value, itl, ttft, rho, max_arrv;

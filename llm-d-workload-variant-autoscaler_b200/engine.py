@@ -8,6 +8,7 @@ entry points they replace:
     update_servers   AddServerInfoToSystemData    internal/utils/utils.go:204 (loads + current allocations)
     recalculate      System.Calculate, for the servers update_servers / update_server_set changed
     update_server_set  System.AddServerFromSpec / RemoveServer   pkg/core/system.go:160 (the whole server set)
+    update_tables    accelerator costs + ModelAcceleratorPerfData, for the (server, accelerator) pairs that read them
     solve            Manager.Optimize             pkg/manager/manager.go:21
     candidates       Server.AllAllocations        pkg/core/server.go:138
     solution         System.GenerateSolution      pkg/core/system.go:303
@@ -97,6 +98,7 @@ def load_library():
     L.wva_update_servers.argtypes = [ctxp] + [C.c_void_p] * len(abi.CYCLE_ARRAYS)
     L.wva_recalculate.argtypes = [ctxp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.wva_update_server_set.argtypes = [ctxp, C.c_int32, C.c_void_p, C.POINTER(abi.System)]
+    L.wva_update_tables.argtypes = [ctxp, C.POINTER(abi.System), C.POINTER(C.c_int64)]
     L.wva_solve.argtypes = [ctxp]
     L.wva_get_candidates.argtypes = [ctxp, C.POINTER(abi.Candidates)]
     L.wva_set_candidates.argtypes = [ctxp, C.POINTER(abi.Candidates)]
@@ -131,7 +133,7 @@ def load_library():
 
 
 EXPORTS = ["wva_set_option", "wva_create", "wva_destroy", "wva_strerror", "wva_last_error", "wva_launch_count",
-           "wva_load_system", "wva_calculate", "wva_update_servers", "wva_recalculate", "wva_update_server_set", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
+           "wva_load_system", "wva_calculate", "wva_update_servers", "wva_recalculate", "wva_update_server_set", "wva_update_tables", "wva_solve", "wva_get_candidates", "wva_set_candidates", "wva_get_solution",
            "wva_analyze_grid", "wva_grid_run", "wva_grid_fetch", "wva_grid_update", "wva_mm1k_eval", "wva_saturation_v1",
            "wva_saturation_upload", "wva_saturation_run", "wva_saturation_fetch", "wva_limit", "wva_saturation_v2",
            "wva_cost_aware_optimize", "wva_enforce", "wva_pipeline_v2", "wva_host_alloc", "wva_host_free", "wva_last_timing",
@@ -287,6 +289,18 @@ class Engine:
         lo, hi = C.c_int32(), C.c_int32()
         self._check(self.lib.wva_comm_shard(self.ctx, C.byref(lo), C.byref(hi)), "wva_comm_shard")
         self.lo, self.hi = lo.value, hi.value
+
+    def update_tables(self, sysd: dict):
+        """The loaded system's accelerator columns (acc_cost, acc_multiplicity, acc_type) and perf_* tables replaced in
+        place by those of `sysd` (its n_acc, n_types and n_models must be the loaded ones; its servers, type_count and
+        optimizer fields are ignored).  The (server, accelerator) pairs whose perf row or accelerator cost changed are
+        re-sized by the next recalculate() and re-evaluated by the next grid_update().  Returns the number of pairs of
+        this context's block this call marks for re-sizing."""
+        st, keep = abi.make_system({**sysd, "n_servers": 0,   # the loaded servers stay
+                                    **{k: np.zeros(0, dt) for k, (dt, e) in abi.SYSTEM_ARRAYS.items() if e == "S"}})
+        n = C.c_int64()
+        self._check(self.lib.wva_update_tables(self.ctx, C.byref(st), C.byref(n)), "wva_update_tables")
+        return n.value
 
     def solve(self):
         self._check(self.lib.wva_solve(self.ctx), "wva_solve")

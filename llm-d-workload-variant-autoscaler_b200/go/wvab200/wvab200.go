@@ -172,6 +172,70 @@ func (x *Ctx) UpdateServerSet(prev []int32, cols *ServerColumns) error {
 	return x.err(C.wva_update_server_set(x.c, C.int32_t(n), p32(prev), &sys), "wva_update_server_set")
 }
 
+// TableColumns are the accelerator columns ([A], accelerator index order) and the perf tables ([M*A], row-major by
+// model) of a wva_system.
+type TableColumns struct {
+	AccCost                                       []float32
+	AccMultiplicity, AccType                      []int32
+	PerfAlpha, PerfBeta, PerfGamma                []float32
+	PerfMaxBatch, PerfAtTokens, PerfAccCount      []int32
+	PerfPresent                                   []uint8
+}
+
+// UpdateTables replaces the accelerator costs, multiplicities and types and the ModelAcceleratorPerfData of the loaded
+// system in place; nAcc, nTypes and nModels must be the loaded ones (a change of shape is a reload).  Recalculate and
+// GridUpdate then re-size and re-evaluate only the (server, accelerator) pairs that read a changed row (INTEGRATION.md
+// §3, per-cycle use).  It returns how many pairs of this context's block the call marked for re-sizing.
+// COMPILE-UNVERIFIED, like the rest of this file.
+func (x *Ctx) UpdateTables(nAcc, nTypes, nModels int, t *TableColumns) (marked int64, err error) {
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread()
+	for _, l := range []int{len(t.AccCost), len(t.AccMultiplicity), len(t.AccType)} {
+		if l != nAcc {
+			return 0, fmt.Errorf("UpdateTables: an accelerator column's length differs from nAcc")
+		}
+	}
+	for _, l := range []int{len(t.PerfAlpha), len(t.PerfBeta), len(t.PerfGamma), len(t.PerfMaxBatch), len(t.PerfAtTokens),
+		len(t.PerfAccCount), len(t.PerfPresent)} {
+		if l != nModels*nAcc {
+			return 0, fmt.Errorf("UpdateTables: a perf column's length differs from nModels * nAcc")
+		}
+	}
+	var pin runtime.Pinner // C copies the columns before returning
+	defer pin.Unpin()
+	p32 := func(s []int32) *C.int32_t {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.int32_t)(unsafe.Pointer(&s[0]))
+	}
+	pf := func(s []float32) *C.float {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.float)(unsafe.Pointer(&s[0]))
+	}
+	pu := func(s []uint8) *C.uint8_t {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.uint8_t)(unsafe.Pointer(&s[0]))
+	}
+	sys := C.wva_system{
+		n_acc: C.int32_t(nAcc), n_types: C.int32_t(nTypes), n_models: C.int32_t(nModels),
+		acc_cost: pf(t.AccCost), acc_multiplicity: p32(t.AccMultiplicity), acc_type: p32(t.AccType),
+		perf_alpha: pf(t.PerfAlpha), perf_beta: pf(t.PerfBeta), perf_gamma: pf(t.PerfGamma),
+		perf_max_batch: p32(t.PerfMaxBatch), perf_at_tokens: p32(t.PerfAtTokens), perf_acc_count: p32(t.PerfAccCount),
+		perf_present: pu(t.PerfPresent),
+	}
+	var n C.int64_t
+	err = x.err(C.wva_update_tables(x.c, &sys, &n), "wva_update_tables")
+	return int64(n), err
+}
+
 // index maps built from SORTED names: ascending index is then a valid Go map order and the
 // name-based tie-breaks of the reference become index comparisons.
 type index struct {

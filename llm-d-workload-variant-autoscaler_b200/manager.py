@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from ._abi import CYCLE_ARRAYS
+from ._abi import CYCLE_ARRAYS, SYSTEM_ARRAYS
 
 # pkg/config/defaults.go:24-33
 DEFAULT_SERVICE_CLASS_NAME = "Free"
@@ -133,13 +133,13 @@ def flatten_spec(spec: dict):
     return d, idx
 
 
-def differs_only_in_cycle_columns(old: dict, new: dict) -> bool:
-    """True when two flattened specs describe the same system up to the per-cycle server columns (loads and current
-    allocations, CYCLE_ARRAYS): every other array equal byte for byte, every scalar equal."""
+def _equal_except(old: dict, new: dict, free) -> bool:
+    """True when two flattened specs have the same keys and every array and scalar not named in `free` is equal (arrays
+    byte for byte, with the same dtype and shape)."""
     if old.keys() != new.keys():
         return False
     for k, a in old.items():
-        if k in CYCLE_ARRAYS:
+        if k in free:
             continue
         b = new[k]
         if isinstance(a, np.ndarray) or isinstance(b, np.ndarray):
@@ -149,6 +149,29 @@ def differs_only_in_cycle_columns(old: dict, new: dict) -> bool:
         elif a != b:
             return False
     return True
+
+
+def differs_only_in_cycle_columns(old: dict, new: dict) -> bool:
+    """True when two flattened specs describe the same system up to the per-cycle server columns (loads and current
+    allocations, CYCLE_ARRAYS): every other array equal byte for byte, every scalar equal."""
+    return _equal_except(old, new, CYCLE_ARRAYS)
+
+
+# the accelerator columns and the perf tables: what Engine.update_tables replaces in place
+TABLE_ARRAYS = tuple(k for k, (dt, e) in SYSTEM_ARRAYS.items() if e in ("A", "MA"))
+
+
+def differs_only_in_tables(old: dict, new: dict) -> bool:
+    """True when two flattened specs describe systems of the same shape (accelerators, types, models, servers) that
+    differ only in the accelerator columns and perf tables (TABLE_ARRAYS: costs, multiplicities, types, perf data) and
+    the per-cycle server columns: Engine.update_tables (+ update_servers) brings the device from one to the other."""
+    for k in TABLE_ARRAYS:
+        if k not in old or k not in new:
+            return False
+        a, b = np.asarray(old[k]), np.asarray(new[k])
+        if a.dtype != b.dtype or a.shape != b.shape:
+            return False
+    return _equal_except(old, new, set(TABLE_ARRAYS) | set(CYCLE_ARRAYS))
 
 
 def server_set_prev(old_index: SpecIndex, old: dict, new_index: SpecIndex, new: dict):
@@ -209,14 +232,20 @@ class Manager:
         """One reconcile cycle on a rebuilt SystemSpec, the same result as `Manager(engine, spec).optimize()`.  When the
         new spec differs from the one on the device only in server loads and current allocations, those columns are
         replaced in place and only the servers they changed are re-sized or re-valued (update_servers -> recalculate
-        -> solve); any other change reloads the system (load_system -> calculate -> solve)."""
+        -> solve).  When accelerator columns or perf data changed too, with the same shapes, the tables are replaced in
+        place first and only the (server, accelerator) pairs that read a changed row are re-sized (update_tables ->
+        update_servers -> recalculate -> solve).  Any other change reloads the system (load_system -> calculate ->
+        solve)."""
         spec = spec["system"] if "system" in spec and "acceleratorData" not in spec else spec
         sysd, index = flatten_spec(spec)
         incremental = self._sized and differs_only_in_cycle_columns(self.sysd, sysd)
+        tables = self._sized and not incremental and differs_only_in_tables(self.sysd, sysd)
         self.spec, self.sysd, self.index, self._cand = spec, sysd, index, None
         self._sized = False
         eng = self.engine
-        if incremental:
+        if incremental or tables:
+            if tables:
+                eng.update_tables(sysd)
             eng.update_servers(*(sysd[k] for k in CYCLE_ARRAYS))
             eng.recalculate()
         else:
