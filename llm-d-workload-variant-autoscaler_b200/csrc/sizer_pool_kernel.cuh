@@ -5,8 +5,9 @@
 // configs[2] (59-62 % with the probe-sorted queue).  Chain length is almost a function of lambda / mu_N alone (early exit
 // E4), and it changes from one bisection step of a pair to the next — so here the binding is dropped:
 //   * a CTA keeps a pool of P pairs whose state (the SizerLane of wva_core.cuh) lives in global memory (L2-resident:
-//     368 bytes per pair); a pair has no head table (m.tab == nullptr): its service rates are computed where a solve
-//     needs them (RateTable, model_rate);
+//     368 bytes per pair, of which a bisection step loads 272 and stores 112: SizerLane's hot block);
+//     a pair has no head table (m.tab == nullptr): its service rates are computed where a solve needs them
+//     (RateTable, model_rate);
 //   * every solve a pair still needs is a REQUEST — the pair's slot — queued in shared memory by class: 28 fast classes
 //     keyed by the head length N (the cost of the certified fast solve, E12) and 4 exact classes keyed by the exact
 //     solver's chain-length estimate, which hold the solves the fast solve did not certify;
@@ -16,8 +17,9 @@
 //     not certify re-queues its pair into an exact class at the same rate; every other lane advances its pair's
 //     bisection / Size / Analyze state machine (sizer_on_solve, the same code as every other sizer), stores the state
 //     back and queues the pair's next request — or retires the pair and frees its slot.
-//   * Free slots are refilled with new pairs from the global work counter: setup runs lane by lane, then the warp scans
-//     the service rates of the lanes that need a model together, 32 entries at a time.
+//   * Free slots are refilled with new pairs from the global work counter, a block of items per warp at a time: setup
+//     runs lane by lane, then the warp scans the service rates of the lanes that need a model together, 32 entries at
+//     a time.
 // Which lanes solve which pairs together changes nothing in any pair's arithmetic: same solves, same order per pair,
 // same state machine — candidates are bit-identical to the lane sizer's (and the oracle's).  tools/proto/lockstep_sim.py
 // and the measured counters (WVA_SIZER_DEBUG) give 88-92 % live lane-steps.
@@ -59,21 +61,41 @@ __device__ __forceinline__ void pool_unlock(int* lock) {
   if ((threadIdx.x & 31) == 0) atomicExch(lock, 0);
 }
 
-// state of a pair <-> the pool (through L2: a slot is rewritten by whichever warp solved it last)
+// state of a pair <-> the pool (through L2: a slot is rewritten by whichever warp solved it last), in 16-byte words
+// [first, end) of the groups SizerLane is laid out in (wva_core.cuh): the model (stored once), the hot block (stored
+// after every solve) and the cold block (stored by the steps that enter or leave the bisection).  The chain's fields but
+// c.states and the dual drivers' fields are never moved: a chain starts and completes within one step.
 static_assert(sizeof(PoolEntry) % 16 == 0 && offsetof(PoolEntry, z) == 0 && offsetof(SizerLane, m) == 0,
               "PoolEntry is copied in 16-byte words, the model first");
 constexpr int POOL_MODEL_WORDS = (int)((sizeof(PairModel) + 15) / 16);
-__device__ __forceinline__ void pool_load(PoolEntry& z, const PoolEntry* e) {
+constexpr int POOL_HOT_FIRST = (int)(offsetof(SizerLane, sT) / 16);
+constexpr int POOL_HOT_END = (int)((offsetof(SizerLane, c) + offsetof(Chain, states) + sizeof(int) + 15) / 16);
+constexpr int POOL_COLD_FIRST = (int)(offsetof(SizerLane, slo_tps) / 16);
+constexpr int POOL_COLD_END = (int)((offsetof(SizerLane, failed) + sizeof(bool) + 15) / 16);
+constexpr bool pool_in(size_t off, int first, int end) { return off >= 16u * first && off < 16u * end; }
+#define POOL_IN(f, g) pool_in(offsetof(SizerLane, f), POOL_##g##_FIRST, POOL_##g##_END)
+static_assert(offsetof(SizerLane, sT) % 16 == 0 && POOL_HOT_FIRST == POOL_MODEL_WORDS && offsetof(Chain, states) == 0 &&
+              POOL_IN(sI, HOT) && POOL_IN(cur_x, HOT) && POOL_IN(stage, HOT) && POOL_IN(solves, HOT) && POOL_IN(states, HOT),
+              "the hot block holds sT, sI, cur_x, stage, solves, states and c.states, and no model word");
+static_assert(offsetof(SizerLane, slo_tps) % 16 == 0 && offsetof(SizerLane, c) + sizeof(Chain) <= offsetof(SizerLane, slo_tps) &&
+              POOL_IN(total_rate, COLD) && POOL_IN(rate_star, COLD) && POOL_IN(acc_cost, COLD) && POOL_IN(srv, COLD) &&
+              POOL_IN(acc, COLD) && POOL_IN(model, COLD) && POOL_IN(min_replicas, COLD) && POOL_IN(n_inst, COLD) &&
+              POOL_IN(split, COLD) && POOL_IN(num_replicas, COLD) && POOL_IN(cost, COLD) && POOL_IN(merged, COLD),
+              "the cold block holds every other field sizer_on_solve and retire_overflow use, and no chain field");
+#undef POOL_IN
+template <int FIRST, int END>
+__device__ __forceinline__ void pool_load(SizerLane& z, const PoolEntry* e) {
   int4* dst = reinterpret_cast<int4*>(&z);
   const int4* src = reinterpret_cast<const int4*>(e);
 #pragma unroll
-  for (int k = 0; k < (int)(sizeof(PoolEntry) / 16); k++) dst[k] = __ldcg(src + k);
+  for (int k = FIRST; k < END; k++) dst[k] = __ldcg(src + k);
 }
-__device__ __forceinline__ void pool_store(PoolEntry* e, const PoolEntry& z) {
+template <int FIRST, int END>
+__device__ __forceinline__ void pool_store(PoolEntry* e, const SizerLane& z) {
   const int4* src = reinterpret_cast<const int4*>(&z);
   int4* dst = reinterpret_cast<int4*>(e);
 #pragma unroll
-  for (int k = 0; k < (int)(sizeof(PoolEntry) / 16); k++) __stcg(dst + k, src[k]);
+  for (int k = FIRST; k < END; k++) __stcg(dst + k, src[k]);
 }
 // what a solve needs of the pair: its queue model and the arrival rate (the rest is re-read after the solve, so that the
 // solver's registers are not shared with 300 bytes of bisection state)
@@ -122,6 +144,9 @@ enum {
   PH_ROWS, PH_ITERS,
   PH_MODEL,                                                       // cycles of fast batches: model load (pool_load_model),
   PH_FAST_WAIT0, PH_FAST_CHUNKS, PH_FAST_FINISH,                  // first table preparation, head chunks, fast_solve_finish
+  PH_ST_LOAD, PH_ST_MACHINE, PH_ST_STORE,                         // cycles of the state phase: slot load, state machine, store
+  PH_NEW_CLAIM, PH_NEW_SCAN, PH_NEW_BEGIN,                        // of the new-pair phase: claim + sizer_setup, rate scan,
+                                                                  // sizer_begin + store
   PH_N
 };
 __device__ unsigned long long g_pool_phase[PH_N];
@@ -261,29 +286,43 @@ sizer_pool_kernel(SysView s, CandView out, const int* list, unsigned long long n
     pushA = pushB = freeA = freeB = -1;
     if (finished) break;
 
-    // ---- new pairs into the reserved slots: setup lane by lane (nil and zero-load pairs need no model), then
-    //      BuildModel (queueanalyzer.go:95-124) with the whole warp, one pair's rates after the other
+    // ---- new pairs into the reserved slots: the lanes that hold one claim a block of work items with one atomicAdd and
+    //      take one item each; an item decided without a solve (nil, zero load, no perf row, over the batch limit) is
+    //      consumed there and its lane claims again with the others left without a pair.  Setup runs lane by lane,
+    //      then BuildModel (queueanalyzer.go:95-124) with the whole warp, one pair's rates after the other
     if (__any_sync(full, new_slot >= 0)) {
       POOL_PH(const unsigned ph_new = __ballot_sync(full, new_slot >= 0); POOL_PH_ADD(PH_ROWS, __popc(ph_new));)
       PoolEntry ze;
       SizerLane& z = ze.z;
       bool need_table = false;
-      if (new_slot >= 0) {
-        while (true) {
-          const unsigned long long item = atomicAdd(&ctr->next_pair, 1ull);
-          if (item >= n_pairs) { sm.exhausted = 1; break; }
-          const unsigned long long pair = list_pair(list, item);
-          const int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
-          int lim = 0;
-          const int rc = sizer_setup(z, s, out, srv, acc, nmax, &lim, true);
-          if (lim) ctr->limit_hit = 1;
-          if (rc == SETUP_NEEDS_TABLE) { need_table = true; break; }
+      for (unsigned want = __ballot_sync(full, new_slot >= 0); want;) {
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(&ctr->next_pair, (unsigned long long)__popc(want));
+        base = __shfl_sync(full, base, 0);
+        bool again = false;
+        if ((want >> lane) & 1u) {
+          const unsigned long long item = base + __popc(want & lt);
+          if (item >= n_pairs) sm.exhausted = 1;
+          else {
+            const unsigned long long pair = list_pair(list, item);
+            const int srv = (int)(pair / (unsigned)s.n_acc), acc = (int)(pair % (unsigned)s.n_acc);
+            int lim = 0;
+            const int rc = sizer_setup(z, s, out, srv, acc, nmax, &lim, true);
+            if (lim) ctr->limit_hit = 1;
+            need_table = rc == SETUP_NEEDS_TABLE;
+            again = !need_table;
+          }
         }
+        want = __ballot_sync(full, again);
       }
+      POOL_PH(__syncwarp(); POOL_PH_ADD(PH_NEW_CLAIM, clock64() - ph_t); long long ph_u = clock64();)
       // each pair's rates: lane l computes entries l, l + 32, ... and keeps none of them; the rate range needs the first
       // and last entry, the monotone region the LAST descent !(row[n-1] <= row[n]) (where model_finish's scan from the
       // top stops): a max over n, and e1_ok whether every entry is an (E1) divisor: an and over n (model_finish checks
-      // the entries below mono and the two ends of the non-decreasing rest, which bound every entry between them)
+      // the entries below mono and the two ends of the non-decreasing rest, which bound every entry between them).
+      // The rates are formed with div_rate, as the solves' RateTable forms them, where every quotient is an (E1)
+      // divisor: den(N) < 2^126 and den(1) >= 2^-109, so that n / den(n) lies in [2^-126, 2^125] for n <= N <= 2^16
+      // (rate_den is monotone); there serv_rate_e1 gives serv_rate's bits without the IEEE division's slow path
       float r0 = 0.0f, rl = 0.0f;
       int mono = 0, e1_ok = 0;
       unsigned need = __ballot_sync(full, need_table);
@@ -291,12 +330,19 @@ sizer_pool_kernel(SysView s, CandView out, const int* list, unsigned long long n
         const int src = __ffs(need) - 1;
         need &= need - 1;
         const PairModel b = shfl_model(z.m, src);
+        const RateCoef bc = rate_coef(b);
+        const bool den_ok = rate_den_ok(rate_den(bc, (float)b.N));
+        const bool e1_div = den_ok && rate_den(bc, 1.0f) >= 0x1p-109f;
         float cur = 0.0f, carry = 0.0f, first = 0.0f;
         int desc = 0;
         bool e1 = true;
         for (int n0 = 0; n0 < b.N; n0 += 32) {
           const int n = n0 + lane;
-          if (n < b.N) { cur = serv_rate(b, n + 1); e1 = e1 && e1_divisor(cur); }
+          if (n < b.N) {
+            const float nf = (float)(n + 1);
+            cur = e1_div ? serv_rate_e1(bc, nf) : serv_rate_nf(bc, nf);
+            e1 = e1 && e1_divisor(cur);
+          }
           float prev = __shfl_up_sync(full, cur, 1);
           if (lane == 0) prev = carry;
           if (n > 0 && n < b.N && !(prev <= cur)) desc = n;
@@ -306,9 +352,10 @@ sizer_pool_kernel(SysView s, CandView out, const int* list, unsigned long long n
         const float last = __shfl_sync(full, cur, (b.N - 1) & 31);
         desc = __reduce_max_sync(full, desc);
         // and the solves' RateTable may form the rates with div_rate: den(N) bounds every denominator
-        const bool all_e1 = __all_sync(full, e1) && rate_den_ok(rate_den(rate_coef(b), (float)b.N));
+        const bool all_e1 = __all_sync(full, e1) && den_ok;
         if (lane == src) { r0 = first; rl = last; mono = desc; e1_ok = all_e1; }
       }
+      POOL_PH(POOL_PH_ADD(PH_NEW_SCAN, clock64() - ph_u); ph_u = clock64();)
       bool live = false;
       if (need_table) {
         PairModel& m = z.m;
@@ -323,9 +370,15 @@ sizer_pool_kernel(SysView s, CandView out, const int* list, unsigned long long n
         if (live && !m.e1_ok) live = pool_pair_on_chain(ze, s, out, ctr, overflow_list, my_states);
         if (!live) my_solves += z.solves;
       }
-      if (live) { pool_store(pool + new_slot, ze); pushB = new_slot; clsB = pool_class(z.m); }
+      if (live) {
+        PoolEntry* e = pool + new_slot;
+        pool_store<0, POOL_HOT_END>(e, z);
+        pool_store<POOL_COLD_FIRST, POOL_COLD_END>(e, z);
+        pushB = new_slot; clsB = pool_class(z.m);
+      }
       else if (new_slot >= 0) freeB = new_slot;
       __syncwarp();
+      POOL_PH(POOL_PH_ADD(PH_NEW_BEGIN, clock64() - ph_u);)
     }
     POOL_PH(POOL_PH_ADD(PH_NEW, clock64() - ph_t); ph_t = clock64();)
 
@@ -376,28 +429,46 @@ sizer_pool_kernel(SysView s, CandView out, const int* list, unsigned long long n
       atomicAdd(&ctr->certify_fallbacks, 1ull);
       __stcg(&pool[my_slot].z.c.states, sv);
       pushA = my_slot; clsA = pool_exact_class(pm.m, x);
-    } else if (live) {
-      PoolEntry ze;
-      SizerLane& z = ze.z;
-      pool_load(ze, pool + my_slot);
+    }
+    // the pair's state: the model, the hot and the cold block (loading the cold block only where a step needs it costs
+    // the loop registers and spills); a step within the bisection (SZ_SEARCH before and after) changes only the hot block
+    const bool step = live && !requeue;
+    PoolEntry* const e = pool + (step ? my_slot : 0);
+    SizerLane z;
+    bool cont = false;
+    int stage0 = SZ_SEARCH;
+    POOL_PH(__syncwarp(); long long ph_u = clock64();)
+    if (step) {
+      pool_load<0, POOL_HOT_END>(z, e);
+      pool_load<POOL_COLD_FIRST, POOL_COLD_END>(z, e);
+      stage0 = z.stage;
+    }
+    POOL_PH(__syncwarp(); POOL_PH_ADD(PH_ST_LOAD, clock64() - ph_u); ph_u = clock64();)
+    if (step) {
       if (!uniform) {                                  // mixed N in the batch: the per-lane state machine
         const int s0 = z.c.states;
+        chain_start_pair(z.c, z.m, z.cur_x);           // the chain lane_start_solve started
+        z.c.states = s0;
         while (!chain_step(z.c, z.m, st)) {}
         bad = z.c.phase == CH_OVERFLOW;
         sv = z.c.states - s0;
       } else {
         z.c.states = exact ? z.c.states + sv : sv;
       }
-      bool cont;
-      if (bad) {
-        retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
-        cont = false;
-      } else {
-        cont = sizer_on_solve(z, s, out, st);
-      }
-      if (cont) { pool_store(pool + my_slot, ze); pushA = my_slot; clsA = pool_class(z.m); }
-      else { my_solves += z.solves; my_states += z.states; freeA = my_slot; }
+      if (bad) retire_overflow(z, s, out, ctr, overflow_list, z.c.states);
+      else cont = sizer_on_solve(z, s, out, st);
     }
+    POOL_PH(__syncwarp(); POOL_PH_ADD(PH_ST_MACHINE, clock64() - ph_u); ph_u = clock64();)
+    if (step) {
+      if (cont) {
+        pool_store<POOL_HOT_FIRST, POOL_HOT_END>(e, z);
+        if (stage0 != SZ_SEARCH || z.stage != SZ_SEARCH) pool_store<POOL_COLD_FIRST, POOL_COLD_END>(e, z);
+        pushA = my_slot; clsA = pool_class(z.m);
+      } else {
+        my_solves += z.solves; my_states += z.states; freeA = my_slot;
+      }
+    }
+    POOL_PH(__syncwarp(); POOL_PH_ADD(PH_ST_STORE, clock64() - ph_u);)
     {
       int mxs = sv;
       for (int o = 16; o; o >>= 1) mxs = max(mxs, __shfl_xor_sync(full, mxs, o));

@@ -301,17 +301,17 @@ struct SolveStats {  // float32 results of computeStatistics (mm1modelstatedepen
 enum { CH_IDLE = 0, CH_PASS1 = 1, CH_PASS2 = 2, CH_DONE = 3, CH_OVERFLOW = 4 };
 
 struct Chain {
+  int states;              // states visited (instrumentation); first: the pool sizer keeps it with SizerLane's hot fields
+  float lambda;
+  int n;                   // index of the state held in p
+  int phase;
   double lam, lamg;        // float64(lambda); lambda*(1+1e-6) guard for the monotone test
   double p;                // unnormalised p~[n]
   double sum, rsum;        // pass-1 total and its correctly rounded reciprocal
   double L, sumP, Lserv;   // pass-2 accumulators (avgNumInSystem, sumP, avgNumInServers)
   double pK;               // normalised p[K]
-  float lambda;
-  int n;                   // index of the state held in p
-  int phase;
   bool tail_ok;            // lambda guard <= mu_last: terms are non-increasing on the tail
   bool sum_ok;             // sum inside the exponent window
-  int states;              // states visited (instrumentation)
 };
 
 WVA_HD void chain_start(Chain& c, float lambda) {
@@ -323,6 +323,11 @@ WVA_HD void chain_start(Chain& c, float lambda) {
   c.n = 0;
   c.phase = CH_PASS1;
   c.states = 0;
+}
+// a chain of pair m at arrival rate lambda
+WVA_HD void chain_start_pair(Chain& c, const PairModel& m, float lambda) {
+  chain_start(c, lambda);
+  c.tail_ok = d_bits(c.lamg) <= d_bits(m.mu_last);
 }
 
 // p~[n+1] = p~[n]*lambda / mu_min(n,N-1)   (mm1modelstatedependent.go:77-83)
@@ -731,26 +736,32 @@ struct Search {   // one BinarySearch (utils.go:26-70)
   bool increasing;
 };
 
+// The fields are grouped by how often a solve touches them, for the pool sizer (sizer_pool_kernel.cuh), which keeps a
+// pair's SizerLane in global memory and copies it in 16-byte words: the model (read before every solve, never changed
+// after sizer_begin), the hot block from sT to c.states (what a bisection step reads and writes), the chain's other
+// fields (a chain starts and ends within one step), the cold block from slo_tps to failed (Size()'s tail and
+// CreateAllocation), and the dual drivers' fields.
 struct SizerLane {
   PairModel m;
-  Chain c;
-  Search sT, sI;          // TTFT and ITL searches
-  float slo_tps, total_rate, rate_star, acc_cost;
+  alignas(16) Search sT;  // TTFT and ITL searches
+  Search sI;
   float cur_x;
-  float x2[2];           // dual driver: the (up to) two arrival rates of the coming round
-  bool act2[2];
-  int i_chain;           // dual driver: chain that carries the ITL search's point
   int stage;
+  int solves;
+  long long states;
+  Chain c;
+  float slo_tps, total_rate, rate_star, acc_cost;
   int srv, acc, model;
   int min_replicas, n_inst;
-  int solves;
   // split mode (lane sizer on mid-size systems): a pair is two work items, one per search; the item that
   // finishes second merges the partner's result and runs the two Analyze solves
   int split;             // -1 whole pair, 0 TTFT item, 1 ITL item
-  bool merged, failed;
-  long long states;
   long long num_replicas;
   float cost;
+  bool merged, failed;
+  float x2[2];           // dual driver: the (up to) two arrival rates of the coming round
+  bool act2[2];
+  int i_chain;           // dual driver: chain that carries the ITL search's point
 };
 
 // result of setup()
@@ -828,8 +839,7 @@ WVA_HD int sizer_setup(SizerLane& z, const SysView& s, const CandView& out, int 
 }
 
 WVA_HD void lane_start_solve(SizerLane& z, float lambda) {
-  chain_start(z.c, lambda);
-  z.c.tail_ok = d_bits(z.c.lamg) <= d_bits(z.m.mu_last);
+  chain_start_pair(z.c, z.m, lambda);
   z.cur_x = lambda;
   z.solves++;
 }
@@ -1153,7 +1163,8 @@ WVA_HD void spec_walk(Search& q, int depth, GetY get_y) {
   }
 }
 
-// The solve at z.cur_x completed with stats st.  Returns false when the pair is finished.
+// The solve at z.cur_x completed with stats st.  Returns false when the pair is finished.  A bisection step that
+// starts another solve (stage SZ_SEARCH before and after) writes only SizerLane's hot block and the chain.
 WVA_HD bool sizer_on_solve(SizerLane& z, const SysView& s, const CandView& out, const SolveStats& st) {
   z.states += z.c.states;
   const PairModel& m = z.m;

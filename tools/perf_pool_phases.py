@@ -5,6 +5,9 @@ System.Calculate on the pool sizer and prints each phase's share of the warps' c
 lane-steps of fast and exact batches.  The fast batches are split further into the model load (pool_load_model), the
 first table preparation of each head pass (a shared-memory tile wait when the rates were streamed from rows), the head chunks (the later tile waits included) and fast_solve_finish, and the head
 chunks' cycles are given per warp-state (one state index of a batch: 32 lane-steps, live or not) and per live lane-state.
+The state phase is split into the slot load, the state machine and the slot store, and the new-pair phase into the
+claim with sizer_setup, the BuildModel rate scan, and sizer_begin with the first store; each part ends at a __syncwarp,
+so a load's latency falls in the part that first waits for its data.
 The product library in the tree is neither used nor touched.
 
 Usage: perf_pool_phases.py [--root TREE] [--out DIR] [--scale S] [--runs R] [--json FILE]
@@ -23,12 +26,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = "llm-d-workload-variant-autoscaler_b200"
 NAMES = ["lock", "new_pairs", "fast", "exact", "state", "total", "fast_batches", "fast_states", "fast_slots",
          "exact_batches", "exact_states", "exact_slots", "fast_partial", "exact_partial", "rows", "iters",
-         "model", "fast_wait0", "fast_chunks", "fast_finish"]
+         "model", "fast_wait0", "fast_chunks", "fast_finish", "state_load", "state_machine", "state_store",
+         "new_claim", "new_scan", "new_begin"]
 PHASES = {"lock": "critical section", "new_pairs": "new-pair setup + BuildModel",
           "fast": "model load + fast head + finish", "exact": "exact solves",
           "state": "state load + sizer_on_solve + store"}
 FAST_PARTS = {"model": "model load", "fast_wait0": "first table preparation", "fast_chunks": "head chunks",
               "fast_finish": "fast_solve_finish"}
+STATE_PARTS = {"state_load": "state load", "state_machine": "sizer_on_solve (mixed-N chains included)",
+               "state_store": "state store"}
+NEW_PARTS = {"new_claim": "claim + sizer_setup", "new_scan": "BuildModel rate scan",
+             "new_begin": "sizer_begin + store"}
 
 
 def build(tree: str, out: str) -> str:
@@ -92,6 +100,13 @@ def main():
     for k, txt in FAST_PARTS.items():
         print(f"    {txt:<38s} {100 * parts[k]:6.2f} %")
     print(f"    {'rest (call, batch bookkeeping)':<38s} {100 * parts['fast_other']:6.2f} %")
+    for name, group, whole in (("state", STATE_PARTS, "state"), ("new pairs", NEW_PARTS, "new_pairs")):
+        sub = {k: r[k] / tot for k in group}
+        res[name.replace(" ", "_") + "_parts"] = sub
+        print(f"  of which, {name}:")
+        for k, txt in group.items():
+            print(f"    {txt:<38s} {100 * sub[k]:6.2f} %")
+        print(f"    {'rest':<38s} {100 * (share[whole] - sum(sub.values())):6.2f} %")
     warp_states = r["fast_slots"] / 32
     res["chunk_cycles_per_warp_state"] = r["fast_chunks"] / max(warp_states, 1)
     res["chunk_cycles_per_live_lane_state"] = r["fast_chunks"] / max(r["fast_states"], 1)
